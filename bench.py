@@ -54,7 +54,29 @@ def parse():
                     help="engine A/B option (Engine.set_option), e.g. --opt pdl=1 with SGMSE_B200_PDL=1; recorded in config")
     ap.add_argument("--no-cpu-baseline", action="store_true")
     ap.add_argument("--no-roofline", action="store_true")
-    return ap.parse_args()
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="after the timed steps, write the enhanced waveforms of the last timed step as DIR/enhanced.npy "
+                         "(float32 [utterances, samples] of all ranks; same arguments -> same inputs, so two builds can be compared). "
+                         "Above 64 MB a fixed, seeded sample of utterances is written, their indices in DIR/enhanced_rows.npy")
+    a = ap.parse_args()
+    if a.dump_outputs and a.impl == "reference":
+        ap.error("--dump-outputs applies to the GPU arm only (--impl b200)")
+    return a
+
+
+DUMP_LIMIT_BYTES = 64 << 20
+
+
+def dump_outputs(dirname, out):
+    """out: float32 [utterances, samples] on the host.  Writes enhanced.npy and enhanced_rows.npy (float64 row indices); when
+    all rows exceed DUMP_LIMIT_BYTES, only a sample of rows drawn with a fixed seed, so the same arguments dump the same rows."""
+    import numpy as np
+    n, length = out.shape
+    k = min(n, DUMP_LIMIT_BYTES // (length * 4 + 8))
+    rows = np.arange(n) if k == n else np.sort(np.random.default_rng(0).choice(n, size=k, replace=False))
+    os.makedirs(dirname, exist_ok=True)
+    np.save(os.path.join(dirname, "enhanced.npy"), np.ascontiguousarray(out[rows], dtype=np.float32))
+    np.save(os.path.join(dirname, "enhanced_rows.npy"), rows.astype(np.float64))
 
 
 def peaks():
@@ -63,7 +85,8 @@ def peaks():
         d = json.load(open(p))
         return {"hbm_gbs": d["hbm_gbs"], "tflops_burst": d["bf16_tflops"], "tflops_sustained": d["bf16_tflops_sustained"],
                 "source": "MEASURED_PEAKS.json"}
-    return {"hbm_gbs": 6650.0, "tflops_burst": 1590.0, "tflops_sustained": 1400.0, "source": "fallback (B200_PROFILING.md)"}
+    # NVIDIA H100 SXM data sheet (700 W card): 3.35 TB/s HBM3, 989 TFLOP/s dense FP16; a data-sheet rate, not a measured one
+    return {"hbm_gbs": 3350.0, "tflops_burst": 989.0, "tflops_sustained": 989.0, "source": "fallback (H100 SXM data sheet, dense FP16)"}
 
 
 # ------------------------------------------------------------------------------------------------
@@ -121,9 +144,8 @@ def _thread_candidates():
 def pick_cpu_threads(forward):
     """Thread sweep on the FULL shape of the workload: one warm + one timed score-network evaluation on a
     [1, 2, 256, 512] input per candidate count, ascending; the fastest wins.  More threads are NOT faster for this
-    batch-1 network (MKL-DNN convolutions: 16 threads 3.75 s, 64 threads 5.3 s, 128 threads 73 s per evaluation on the
-    128-CPU host of the B200 box, profiles/r02_bench_reference_arm.json), so the sweep stops once two candidates in a row are
-    slower than the best so far or one is more than 1.25x slower: the 128-thread point alone would cost 2.5 minutes.  The table goes into the JSON line (`cpu_baseline.thread_sweep_s_per_forward`)."""
+    batch-1 network (MKL-DNN convolutions scale badly past a few dozen threads on a large host), so the sweep stops once two
+    candidates in a row are slower than the best so far or one is more than 1.25x slower.  The table goes into the JSON line (`cpu_baseline.thread_sweep_s_per_forward`)."""
     if _CPU["threads"] is not None:
         return _CPU["threads"]
     import torch
@@ -139,7 +161,7 @@ def pick_cpu_threads(forward):
             best, worse = (dt, c), 0
         else:
             worse += 1
-            if worse >= 2 or dt > 1.25 * best[0]:      # the curve has turned (3.7 s at 48 threads, 5.1 s at 64, 69 s at 128)
+            if worse >= 2 or dt > 1.25 * best[0]:      # the curve has turned
                 sweep["stopped_after"] = c
                 break
     _CPU.update(threads=best[1], sweep=sweep, forward_s=best[0])
@@ -183,7 +205,7 @@ def cpu_state():
             t3 = time.perf_counter()
             return t3 - t0, (t1 - t0) + (t3 - t2)
         kind = "reference"
-        _CPU["source"] = refshim.reference_kind() + ": " + refshim.REFERENCE_ROOT     # 'staged: .../oracle/_ref' on the GPU box
+        _CPU["source"] = refshim.reference_kind() + ": " + refshim.REFERENCE_ROOT
     else:
         print("bench.py: oracle/_ref is not staged (run __graft_entry__.build() where /root/reference exists): "
               "the CPU arm falls back to the oracle PORT", file=sys.stderr)
@@ -262,11 +284,11 @@ def workload_config(args):
             "global_batch": args.batch * args.gpus, "per_gpu_batch": args.batch, "micro_batch": args.micro_batch, "lanes": args.lanes,
             "parallelism": f"dp{args.gpus} (batch sharded, no data-path collective)",
             **({"options": list(args.opt)} if getattr(args, "opt", None) else {}),
-            "l2": "working set per step (>10 GB of activations per micro-batch) exceeds the 126 MB L2; no flush needed"}
+            "l2": "working set per step (>10 GB of activations per micro-batch) exceeds the 50 MB L2; no flush needed"}
 
 
 # ------------------------------------------------------------------------------------------------
-# B200 arm
+# GPU arm
 # ------------------------------------------------------------------------------------------------
 def run_b200(args):
     import torch
@@ -336,6 +358,13 @@ def run_b200(args):
         clocks.start()
     ms = timed(step_dev, args.steps)
     launches = eng.counter("kernel_launches") - l0
+    if args.dump_outputs:
+        every = out_dev
+        if world > 1:                                   # every rank enhanced its own shard of utterances
+            every = torch.empty((world * args.batch, L), dtype=out_dev.dtype, device=dev)
+            dist.all_gather_into_tensor(every, out_dev)
+        if rank == 0:
+            dump_outputs(args.dump_outputs, every.float().cpu().numpy())
     step_host(0)
     ms_e2e = timed(step_host, args.steps)
     clk = clocks.stop() if rank == 0 else None
@@ -347,7 +376,7 @@ def run_b200(args):
 
     roof = None
     if not args.no_roofline and args.mode == "fp16_tc":
-        # dominant kernels = the tcgen05 implicit-GEMM convolutions: CUDA events around every launch of one more
+        # dominant kernels = the wgmma implicit-GEMM convolutions: CUDA events around every launch of one more
         # (eager, un-graphed) step on the launching stream
         eng.set_option("time_convs", 1)
         step_dev(0)
@@ -374,12 +403,12 @@ def run_b200(args):
             else:
                 traffic_note = {"stale": f"profiles/r02_conv_traffic.json was captured from kernel sources {tj.get('source_digest')}, "
                                          f"this build is {source_digest()}: re-run tools/make_conv_traffic.py"}
-        roof = {"kernel": "tcgen05 implicit-GEMM convolutions (conv_tc6 with fused GroupNorm+SiLU producers; conv_tc4 / conv_tc on the levels below 32 rows)",
+        roof = {"kernel": "wgmma implicit-GEMM convolutions (conv_tc, TMA-fed operands)",
                 "bound": "tensor", "achieved": round(ach, 1),
                 "peak": pk["tflops_sustained"], "unit": "TFLOP/s", "frac": round(ach / pk["tflops_sustained"], 4),
                 "traffic": traffic, "traffic_of": traffic_note,
                 "launches_timed": cnt, "avg_launch_us": round(us / max(cnt, 1), 1),
-                "peak_source": pk["source"] + " (bf16_tflops_sustained: kernel timed inside a long step)",
+                "peak_source": pk["source"],
                 "share_of_step": round(us * 1e-3 / (ms / args.steps), 3),
                 # the same launches against the other roof: algorithmic HBM bytes / time (KB/us = GB/s)
                 "algorithmic_hbm_gbs": round(kbytes / max(us, 1), 1), "hbm_peak_gbs": pk["hbm_gbs"],

@@ -1,4 +1,4 @@
-/* sgmse_b200 — C-ABI of the B200-native reverse-SDE enhancement engine.
+/* sgmse_b200 — C-ABI of the H100-native reverse-SDE enhancement engine.
  *
  * Drop-in boundary for the hot path of sp-uhh/sgmse (SURVEY.md §8b).  Plain C: opaque handle, raw
  * device/host pointers and sizes, int return codes (0 = ok, non-zero = error; the message is available
@@ -54,7 +54,7 @@ typedef struct sgmse_b200_engine sgmse_b200_engine;
 enum { SGMSE_B200_BACKBONE_NCSNPP = 0, SGMSE_B200_BACKBONE_NCSNPP_48K = 1, SGMSE_B200_BACKBONE_NCSNPP_V2 = 2 };
 /* arithmetic mode: 0 = fp32 activations, CUDA-core convolutions (validation);
  *                  1 = fp16 activations, CUDA-core convolutions (debug);
- *                  2 = fp16 activations, tcgen05 tensor-core convolutions (product path) */
+ *                  2 = fp16 activations, wgmma tensor-core convolutions (product path) */
 enum { SGMSE_B200_MODE_FP32 = 0, SGMSE_B200_MODE_FP16_DIRECT = 1, SGMSE_B200_MODE_FP16_TC = 2 };
 enum { SGMSE_B200_PRED_REVERSE_DIFFUSION = 0, SGMSE_B200_PRED_EULER_MARUYAMA = 1, SGMSE_B200_PRED_NONE = 2 };
 enum { SGMSE_B200_CORR_ALD = 0, SGMSE_B200_CORR_LANGEVIN = 1, SGMSE_B200_CORR_NONE = 2 };
@@ -217,21 +217,21 @@ int sgmse_b200_enhance_ode(sgmse_b200_engine* e, const float* wav, int B, int L,
 long long sgmse_b200_workspace_bytes(sgmse_b200_engine* e, int B, int F, int T);
 /* copy a recorded intermediate activation (see sgmse_b200_set_option "record_taps") as fp32 NCHW to host */
 int sgmse_b200_get_tap(sgmse_b200_engine* e, const char* name, float* out_host, long long cap, int shape[4]);
-/* options: "record_taps" (0/1), "use_graphs" (0/1), "tc_mask" (bit i set = conv class i may use tcgen05),
+/* options: "record_taps" (0/1), "use_graphs" (0/1), "tc_mask" (bit i set = conv class i may use the wgmma kernel),
  * "time_convs" (0/1: bracket every convolution launch with CUDA events; disables graph replay),
  * "lanes" (1..8 concurrent launch sequences inside a captured sampler graph), "max_graphs" (captured sampler graphs kept,
  * least recently used evicted; default 16).  The kernel A/B switches the tools use ("tc_variant", "attn_variant",
- * "fir_variant", "inconv_variant", "outconv_variant", "combine_variant", "tc1_narrow", "gn_self", "gnfin_variant", "tc6_*") are
+ * "fir_variant", "inconv_variant", "outconv_variant", "combine_variant", "tc1_narrow", "gn_self", "gnfin_variant") are
  * state of THIS engine: every entry point installs the calling engine's selection before it launches anything, so another
  * engine of the same process (another device, another host thread) never sees them, and a captured sampler graph keeps
- * the selection it was captured with.  Value 0 always selects the current default kernel; since round 2 these are
- * the gated round-2 kernels (strip-mapped conv_tc6 producers, cp.async / prefetched small-end kernels, half2 FIR-up, folded
- * gn_finalize, tcgen05 attention), and the round-1 kernels keep a number of their own: tc6_lean 4, fir_variant 3,
- * outconv_variant 4, inconv_variant 3, combine_variant 2, tc1_narrow / gn_self / gnfin_variant 2, attn_variant 3
+ * the selection it was captured with.  Value 0 always selects the current default kernel (TMA-fed wgmma convolutions,
+ * cp.async / prefetched small-end kernels, half2 FIR-up, folded gn_finalize), and the alternatives keep a number of their
+ * own: tc_variant 5 (GroupNorm+SiLU fused into the convolutions), fir_variant 3, outconv_variant 4, inconv_variant 3,
+ * combine_variant 2, tc1_narrow / gn_self / gnfin_variant 2, attn_variant 3 (plain tile staging)
  * (tests/test_gpu_zz_next_rows.py::test_round1_kernels_agree_with_the_defaults).  No environment variable changes kernel
- * selection.  "tc_variant" 2 / 3 / 5 / 9 / 10 and "tc6_lean" 1 / 4 (superseded convolution generations and producer forms), "tc6_ablate" and "pdl" (0/1: programmatic
- * dependent launch between the kernels of the launch sequence) exist only in the lab twin built with -DSGMSE_B200_PDL
- * (libsgmse_b200_pdl.so, counter "pdl_compiled" = 1); the product library refuses them. */
+ * selection.  "pdl" (0/1: programmatic dependent launch between the kernels of the launch sequence) exists only in the
+ * twin library built with -DSGMSE_B200_PDL (libsgmse_b200_pdl.so, counter "pdl_compiled" = 1); the product library
+ * refuses it. */
 int sgmse_b200_set_option(sgmse_b200_engine* e, const char* key, long long value);
 /* counters: "kernel_launches" (since creation), "graph_launches", "cached_graphs", "workspace_bytes", "weights_bytes",
  * "tc_convs_last_forward", "direct_convs_last_forward", "launches_last_forward",

@@ -1,7 +1,7 @@
 """Architecture walk of the NCSN++ score network (oracle side).
 
 Restates, as a flat list of layer records, the module list the reference builds
-in ``NCSNpp.__init__`` (/root/reference/sgmse/backbones/ncsnpp.py:50-253) and
+in ``NCSNpp.__init__`` (sgmse/backbones/ncsnpp.py:50-253) and
 ``NCSNpp_48k.__init__`` (ncsnpp_48k.py:52-256).  Only the configurations the
 two registered backbones can reach with ``resblock_type='biggan'``,
 ``fir=True``, ``progressive in {'output_skip','none'}`` and

@@ -1,6 +1,6 @@
 """Functional fp32/fp64 restatement of the NCSN++ forward pass (oracle).
 
-Follows /root/reference/sgmse/backbones/ncsnpp.py:256-419 (and ncsnpp_48k.py:259-424
+Follows sgmse/backbones/ncsnpp.py:256-419 (and ncsnpp_48k.py:259-424
 for the ``ncsnpp_48k`` ordering of ``/t`` and ``output_layer``), with the blocks of
 ncsnpp_utils/layerspp.py and the FIR resamplers of up_or_down_sampling.py:195-257 /
 op/upfirdn2d.py:162-203.  Operates on a plain ``{key: tensor}`` state dict in the

@@ -1,6 +1,6 @@
 """Probability-flow ODE sampler (oracle) -- SURVEY.md §8(f-4).
 
-Follows /root/reference/sgmse/sampling/__init__.py:72-143 (``get_ode_sampler``), sdes.py:91-137
+Follows sgmse/sampling/__init__.py:72-143 (``get_ode_sampler``), sdes.py:91-137
 (``RSDE.sde`` with ``probability_flow=True``) and sdes.py:188-196 (``OUVESDE.sde``).
 
 The integrator the reference calls is third-party: ``scipy.integrate.solve_ivp(method='RK45')`` (the reference pins

@@ -1,8 +1,8 @@
 """End-to-end enhancement path (oracle): normalise -> STFT -> compress -> pad -> PC sample
 -> decompress -> iSTFT -> renormalise.
 
-Follows the sequence of /root/reference/sgmse/model.py:426-465 (``ScoreModel.enhance``)
-resp. /root/reference/enhancement.py:75-96, batched over utterances.
+Follows the sequence of sgmse/model.py:426-465 (``ScoreModel.enhance``)
+resp. enhancement.py:75-96, batched over utterances.
 TEST INFRASTRUCTURE – see oracle/__init__.py.
 """
 from __future__ import annotations

@@ -113,7 +113,7 @@ def import_reference(cuda_op: bool = False):
     ``torch.utils.cpp_extension.load`` at import time wherever ``torch.cuda.is_available()``
     (op/upfirdn2d.py:11-20), a minute of nvcc on every fresh GPU box; CUDA is hidden for the duration of the
     first import so CPU tensors take ``upfirdn2d_native`` exactly as in the build container.  cuda_op=True
-    lets the JIT happen (tools/bench_reference_gpu.py: the reference's own GPU path on the same B200)."""
+    lets the JIT happen (the reference's own GPU path)."""
     if not reference_available():
         raise RuntimeError("reference not available at " + REFERENCE_ROOT)
     _install_stubs()

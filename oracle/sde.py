@@ -1,6 +1,6 @@
 """OUVE SDE scalars and the predictor-corrector sampler (oracle).
 
-Follows /root/reference/sgmse/sdes.py:72-89,130-135,188-229,
+Follows sgmse/sdes.py:72-89,130-135,188-229,
 sampling/__init__.py:52-68, sampling/predictors.py:41-76 and
 sampling/correctors.py:37-94.  Noise is *injected* (popped from a list of
 pre-generated complex normals) instead of drawn from torch's global RNG, so that

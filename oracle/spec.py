@@ -1,8 +1,8 @@
 """STFT / iSTFT / magnitude compression / padding (oracle).
 
-Follows /root/reference/sgmse/data_module.py:13-19 (window), :162-188
+Follows sgmse/data_module.py:13-19 (window), :162-188
 (spec_fwd / spec_back, 'exponent' transform), :190-218 (stft / istft kwargs) and
-/root/reference/sgmse/util/other.py:76-90 (pad_spec).  The STFT itself is
+sgmse/util/other.py:76-90 (pad_spec).  The STFT itself is
 restated with an explicit frame matrix + rfft so that the oracle does not share
 ``torch.stft`` with the reference; both are compared in tests/.
 

@@ -12,7 +12,7 @@
 * ``model.get_ode_sampler(y, N=None, minibatch=None, **kw)`` (model.py:370-390; OUVE SDE, score backbones) -> callable
   returning ``(sample, nfe)`` -- the probability-flow ODE with scipy's RK45 restated on the device,
 
-to the B200 engine.  ``sgmse/model.py`` itself is untouched; ``uninstall(model)`` restores the
+to the GPU engine.  ``sgmse/model.py`` itself is untouched; ``uninstall(model)`` restores the
 original bound methods.  The predictor / corrector names are the reference registry names
 (sampling/predictors.py:41,55,68; correctors.py:37,59,84) and unknown names raise the same
 ``ValueError`` as ``Registry.get_by_name`` (util/registry.py:25-30).

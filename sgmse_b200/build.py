@@ -1,10 +1,9 @@
-"""In-tree build of libsgmse_b200.so (nvcc, sm_100a only).
+"""In-tree build of libsgmse_b200.so (nvcc, sm_90a only).
 
     python -m sgmse_b200.build [--force] [--pdl]
 
-The shared library lands in ``sgmse_b200/lib/`` (git-ignored, but it travels to the GPU box with the
-gpurun snapshot).  CUDA runtime is linked statically; cuFFT dynamically (``libcufft.so.11`` from the
-toolkit, rpath'ed).
+The shared library lands in ``sgmse_b200/lib/`` (git-ignored build product).  CUDA runtime is linked
+statically; cuFFT dynamically (``libcufft.so.11`` from the toolkit, rpath'ed).
 """
 from __future__ import annotations
 
@@ -18,20 +17,17 @@ HERE = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(HERE, "csrc")
 LIBDIR = os.path.join(HERE, "lib")
 LIBNAME = "libsgmse_b200.so"
-SOURCES = ["gn.cu", "conv_direct.cu", "conv_tc.cu", "conv_tc4.cu", "conv_tc6.cu", "small.cu", "attn.cu", "attn_umma.cu", "misc.cu", "pack.cu", "ode.cu", "engine.cu"]
-# superseded tcgen05 convolution generations (tc_variant 2 / 3 / 5): kept for the A/B record, compiled into the lab twin only
-LAB_SOURCES = ["conv_tc2.cu", "conv_tc3.cu", "conv_tc5.cu"]
+SOURCES = ["gn.cu", "conv_direct.cu", "conv_tc.cu", "small.cu", "attn.cu", "misc.cu", "pack.cu", "ode.cu", "engine.cu"]
 HEADERS = ["common.cuh", "kernels.h", "engine.h", "rk45.h", os.path.join("..", "..", "include", "sgmse_b200.h")]
 
 NVCC = os.environ.get("NVCC", "/usr/local/cuda/bin/nvcc")
 CUDA_LIB = os.environ.get("CUDA_LIB", "/usr/local/cuda/lib64")
-ARCH = ["-gencode", "arch=compute_100a,code=sm_100a"]
+ARCH = ["-gencode", "arch=compute_90a,code=sm_90a"]
 CFLAGS = ["-O3", "-std=c++17", "-lineinfo", "-Xcompiler", "-fPIC",
           "--expt-relaxed-constexpr", "-diag-suppress", "177"]
 
 
-# the LAB twin: the product sources + LAB_SOURCES with -DSGMSE_B200_PDL (programmatic dependent launch, timing ablations of
-# conv_tc6, the superseded convolution generations); never loaded unless SGMSE_B200_PDL=1
+# the PDL twin: the product sources with -DSGMSE_B200_PDL (programmatic dependent launch); never loaded unless SGMSE_B200_PDL=1
 PDL_LIBNAME = "libsgmse_b200_pdl.so"
 PRODUCT_DEFS: list = []                # see DESIGN.md section 3 (programmatic dependent launch)
 
@@ -43,7 +39,7 @@ def lib_path(pdl: bool = False) -> str:
 def _digest(extra: str = "") -> str:
     h = hashlib.sha256()
     h.update(extra.encode())
-    for f in SOURCES + LAB_SOURCES + HEADERS:
+    for f in SOURCES + HEADERS:
         with open(os.path.join(CSRC, f), "rb") as fh:
             h.update(fh.read())
     h.update(" ".join(ARCH + CFLAGS + PRODUCT_DEFS).encode())
@@ -57,7 +53,7 @@ def build(force: bool = False, verbose: bool = False, pdl: bool = False) -> str:
     stamp = os.path.join(LIBDIR, "build_pdl.stamp" if pdl else "build.stamp")
     dig = _digest("pdl" if pdl else "")
     out = lib_path(pdl)
-    defs = ["-DSGMSE_B200_PDL", "-DSGMSE_B200_LAB"] if pdl else PRODUCT_DEFS
+    defs = ["-DSGMSE_B200_PDL"] if pdl else PRODUCT_DEFS
     if not force and os.path.exists(out) and os.path.exists(stamp) and open(stamp).read() == dig:
         return out
     objdir = os.path.join(LIBDIR, "obj_pdl" if pdl else "obj")
@@ -73,9 +69,8 @@ def build(force: bool = False, verbose: bool = False, pdl: bool = False) -> str:
             print(r.stdout, r.stderr, file=sys.stderr)
         return obj
 
-    sources = SOURCES + (LAB_SOURCES if pdl else [])
-    with concurrent.futures.ThreadPoolExecutor(max_workers=min(8, len(sources))) as ex:
-        objs = list(ex.map(compile_one, sources))
+    with concurrent.futures.ThreadPoolExecutor(max_workers=min(8, len(SOURCES))) as ex:
+        objs = list(ex.map(compile_one, SOURCES))
     cmd = [NVCC, *ARCH, "-shared", "-cudart", "static", "-o", out, *objs,
            "-L" + CUDA_LIB, "-lcufft", "-Xlinker", "-rpath," + CUDA_LIB]
     r = subprocess.run(cmd, capture_output=True, text=True)

@@ -1,6 +1,6 @@
 // Single-head global self-attention over the H*W tokens of one utterance (AttnBlockpp core).
 //
-// Reference: /root/reference/sgmse/backbones/ncsnpp_utils/layerspp.py:82-86
+// Reference: sgmse/backbones/ncsnpp_utils/layerspp.py:82-86
 //   w = softmax_k( sum_c q[c,tok] k[c,key] / sqrt(C) );  h[tok] = sum_key w v[key]
 // 0.16 % of the network FLOPs (SURVEY.md §8a) -> fp32 CUDA-core kernel, smem-tiled; the q/k/v
 // projections and the output projection run through the convolution kernels as 1x1 convs.
@@ -146,8 +146,8 @@ static void run(cudaStream_t st, const TensorDesc& qkv, TensorDesc& out, int S, 
 // ------------------------------------------------------------------------------------------------
 // fp16 tensor-core path (mma.sync m16n8k16, fp32 accumulate), flash-style online softmax.
 // One block = 64 queries of one utterance (4 warps x 16 queries); keys/values stream through smem in tiles of 64.
-// This is the legacy HMMA path on purpose: attention is 0.16 % of the network FLOPs and its tiles (S <= 512 tokens,
-// head dim 128/256) are too small to amortise a TMEM/tcgen05 pipeline; the convolutions own the tcgen05 kernels.
+// mma.sync rather than wgmma on purpose: attention is 0.16 % of the network FLOPs and its tiles (S <= 512 tokens,
+// head dim 128/256) are too small to amortise a warpgroup pipeline; the convolutions own the wgmma kernels.
 // ------------------------------------------------------------------------------------------------
 __device__ __forceinline__ void ldsm_x4(uint32_t (&r)[4], const void* p) {
   asm volatile("ldmatrix.sync.aligned.m8n8.x4.shared.b16 {%0, %1, %2, %3}, [%4];"
@@ -168,9 +168,9 @@ __device__ __forceinline__ uint32_t pack_half2(float lo, float hi) {
 }
 
 namespace {
-// ASYNC (attn_variant 2; gated on a B200 in round 2, bit-identical to the plain staging): Q/K/V tiles are staged with cp.async (zero-fill past the
+// ASYNC (the default; attn_variant 3 selects the plain staging, bit-identical): Q/K/V tiles are staged with cp.async (zero-fill past the
 // last token).  The SASS of the plain load_tile loop is LDG.128 -> STS.128 -> branch, 16 (C = 128) / 32 (C = 256) serialized
-// round trips per tile and two tiles per key block: ~50 us of a 53 us launch whose 4.3 GFLOP need < 10.  Same bytes in
+// round trips per tile and two tiles per key block, i.e. the plain form is latency-bound on its loads.  Same bytes in
 // shared memory, same arithmetic: bit-identical.
 template <int C, bool ASYNC = false>
 __global__ void __launch_bounds__(128) attention_tc_kernel(const __half* __restrict__ qkv, int S, float scale_log2e,
@@ -302,14 +302,11 @@ thread_local int g_attn_variant = 0;   // see kernels.h
 void launch_attention(cudaStream_t st, const TensorDesc& qkv, TensorDesc& out) {
   const int C = out.C, S = qkv.H * qkv.W;
   SG_CHECK(qkv.C == 3 * C && C % 8 == 0, "attention: qkv must have 3C channels");
-  // default: the tcgen05 kernel (attn_umma.cu) where it applies (fp16, C = 256, 128 | tokens <= 512: the three 512-token
-  // blocks of the 16 kHz network at T = 512); the mma.sync kernel below serves the 32-token bottleneck and C = 128
-  if (g_attn_variant == 0 && attention_umma_supported(qkv, out)) { launch_attention_umma(st, qkv, out, nullptr); return; }
-  if (qkv.dt == DT_F16 && g_attn_variant == 2) {
+  if (qkv.dt == DT_F16 && (g_attn_variant == 0 || g_attn_variant == 2)) {
     if (C == 256) { run_tc<256, true>(st, qkv, out, S); return; }
     if (C == 128) { run_tc<128, true>(st, qkv, out, S); return; }
   }
-  if (qkv.dt == DT_F16 && (g_attn_variant == 0 || g_attn_variant == 2 || g_attn_variant == 3)) {
+  if (qkv.dt == DT_F16 && g_attn_variant == 3) {
     if (C == 256) { run_tc<256>(st, qkv, out, S); return; }
     if (C == 128) { run_tc<128>(st, qkv, out, S); return; }
   }

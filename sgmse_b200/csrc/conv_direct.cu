@@ -2,7 +2,7 @@
 //
 // This is the *validation* convolution: fp32 (or fp16-storage) arithmetic with fp32 accumulation,
 // any channel count that is a multiple of 16.  It implements exactly the same contract as the
-// tcgen05 kernel in conv_tc.cu (same K ordering, same epilogue, same statistics side-output), so
+// wgmma kernel in conv_tc.cu (same K ordering, same epilogue, same statistics side-output), so
 // that (a) the engine has an fp32-accurate mode to separate algorithmic from precision error and
 // (b) the tensor-core kernel can be checked against it on the device.
 //

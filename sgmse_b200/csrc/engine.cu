@@ -514,12 +514,11 @@ struct Fwd {
   // coefficients itself and the finalize launch is skipped (the table is still allocated: same workspace either way)
   float2* gn(const TensorDesc& x0, const TensorDesc* x1, long long g_off, long long b_off, bool plain_consumer = false) {
     const int Ct = x0.C + (x1 ? x1->C : 0);
-    // (a, b) as float2 [N][Ct], followed by the half2 table [N][Ct/2] x 16 B of the in-conv producers (ab16_of)
-    float2* ab = (float2*)e.arena.alloc((size_t)x0.N * Ct * 16);
+    // (a, b) as float2 [N][Ct]
+    float2* ab = (float2*)e.arena.alloc((size_t)x0.N * Ct * sizeof(float2));
     const int groups = gn_groups(Ct);
-    uint4* ab16 = (Ct / groups) % 2 == 0 ? (uint4*)(ab + (size_t)x0.N * Ct) : nullptr;
     if (plain_consumer && gn_self_applies(x0, x1)) return ab;
-    if (!dry) { launch_gn_finalize(st, x0, x1, e.blob_dev + g_off, e.blob_dev + b_off, groups, ab, ab16, e.range_flag); count(); }
+    if (!dry) { launch_gn_finalize(st, x0, x1, e.blob_dev + g_off, e.blob_dev + b_off, groups, ab, e.range_flag); count(); }
     return ab;
   }
   // y = [silu](a x + b) without resampling: gn_apply_plain on the finalized table, or (gn_self) finalize + apply in one kernel
@@ -539,18 +538,12 @@ struct Fwd {
     const Resample rs = l.up ? RS_UP : (l.down ? RS_DOWN : RS_NONE);
     const int Ho = l.up ? x0.H * 2 : (l.down ? x0.H / 2 : x0.H);
     const int Wo = l.up ? x0.W * 2 : (l.down ? x0.W / 2 : x0.W);
-    // Fused path (conv_tc5): the 3x3 convs read the RAW tensor and apply GroupNorm+SiLU on the way into shared
-    // memory, so the gn_apply pass (one read + one write of the tensor) and its buffer disappear.
-    const bool fuse_ok = e.cfg.mode == SGMSE_B200_MODE_FP16_TC && (g_tc_variant == 0 || g_tc_variant == 5 || g_tc_variant >= 7);
-#ifdef SGMSE_B200_LAB
-    auto shape_ok = g_tc_variant == 5 ? conv_tc5_shape_ok : conv_tc6_fuse_shape_ok;
-#else
-    auto shape_ok = conv_tc6_fuse_shape_ok;
-#endif
-    const bool fuse0 = fuse_ok && ((e.tc_mask >> 8) & 1) && rs == RS_NONE && l.c0.w_tc && shape_ok(Ho, Wo, x0.C, x1 ? x1->C : 0, l.cout, 0);
-    const int nraw1 = l.shortcut ? ((rs == RS_NONE && x1) ? 2 : 1) : 1;
-    const bool fuse1 = fuse_ok && ((e.tc_mask >> 9) & 1) && l.c1.w_tc && shape_ok(Ho, Wo, l.cout, 0, l.cout, nraw1) &&
-                       (l.shortcut || l.c1.identity_tail);
+    // Fused path (conv_tc, opt-in tc_variant 5): the 3x3 convs read the RAW tensor and apply GroupNorm+SiLU on the way into
+    // shared memory, so the gn_apply pass and its buffer disappear -- but its producer evaluates GroupNorm+SiLU once per tap
+    // (9x the activation work): the benchmark step takes 3.2x longer than with TMA-fed operands and separate gn_apply passes.
+    const bool fuse_ok = e.cfg.mode == SGMSE_B200_MODE_FP16_TC && g_tc_variant == 5;
+    const bool fuse0 = fuse_ok && ((e.tc_mask >> 8) & 1) && rs == RS_NONE && l.c0.w_tc && conv_tc_fuse_shape_ok(Ho, Wo, x0.C, x1 ? x1->C : 0, l.cout);
+    const bool fuse1 = fuse_ok && ((e.tc_mask >> 9) & 1) && l.c1.w_tc && conv_tc_fuse_shape_ok(Ho, Wo, l.cout, 0, l.cout);
     float2* ab0 = gn(x0, x1, l.gn0_w, l.gn0_b, rs == RS_NONE && !fuse0);
     TensorDesc h0;
     TensorDesc xr;                                 // FIR-resampled raw input (up/down blocks)
@@ -569,7 +562,6 @@ struct Fwd {
       a.nseg = 1; a.seg[0].taps = 9;
       if (fuse0) {
         a.seg[0].src = x0; a.gn_ab = ab0;
-        if ((Ct / gn_groups(Ct)) % 2 == 0) a.gn_ab16 = (const uint4*)(ab0 + (size_t)N * Ct);
         if (x1) { a.gn_has_cat = true; a.gn_cat = *x1; }
       } else {
         a.seg[0].src = h0;
@@ -590,7 +582,6 @@ struct Fwd {
       a.nseg = 1; a.seg[0].taps = 9;
       if (fuse1) {
         a.seg[0].src = h1; a.gn_ab = ab1;
-        if ((l.cout / gn_groups(l.cout)) % 2 == 0) a.gn_ab16 = (const uint4*)(ab1 + (size_t)N * l.cout);
       } else { a.seg[0].src = h2; }
       if (l.shortcut) {
         if (rs != RS_NONE) { a.seg[a.nseg].src = xr; a.seg[a.nseg++].taps = 1; }
@@ -1618,7 +1609,6 @@ void enhance_ode(Engine& e, const float* wav, int B, int L, const sgmse_b200_ode
 // Option value 0 always means "the current default kernel".  Round 2 made the gated round-2 candidates the defaults (bit-identical
 // to the round-1 kernels except fir_variant: half2 FIR-up, rel-L2 8e-4 per forward); the round-1 kernels stay selectable under a
 // new number.  The launch helpers keep their internal numbering, the translation lives here:
-//   tc6_lean        0 = strip-mapped producers (internal 2) | 1 = first lean form | 3 = strip + half2 math | 4 = round-1 mode-1 producers
 //   fir_variant     0 = all loads in flight + half2 FIR-up (internal 2) | 1 = expf silu, fp32 FIR | 3 = round-1 kernel
 //   outconv_variant 0 = cp.async staging (internal 3) | 1 = CUDA-core | 2 = fused GroupNorm | 4 = round-1 kernel
 //   inconv_variant  0 = prefetched A fragments (internal 2) | 1 = CUDA-core | 3 = round-1 kernel
@@ -1627,10 +1617,7 @@ void enhance_ode(Engine& e, const float* wav, int B, int L, const sgmse_b200_ode
 static int xl(int v, int new_default, int old_number) { return v == 0 ? new_default : (v == old_number ? 0 : v); }
 static void activate(const sgmse_b200_engine& e) {
   const auto& o = e.opts;
-  sgmse::g_tc_variant = o.tc_variant; sgmse::g_tc6_rings = o.tc6_rings;
-  sgmse::g_tc6_mma_style = o.tc6_mma; sgmse::g_tc6_tma_poll = o.tc6_tma_poll; sgmse::g_tc6_roles = o.tc6_roles;
-  sgmse::g_tc6_ablate = o.tc6_ablate; sgmse::g_attn_variant = o.attn_variant;
-  sgmse::g_tc6_lean = xl(o.tc6_lean, 2, 4);
+  sgmse::g_tc_variant = o.tc_variant; sgmse::g_attn_variant = o.attn_variant;
   sgmse::g_fir_variant = xl(o.fir_variant, 2, 3);
   sgmse::g_outconv_variant = xl(o.outconv_variant, 3, 4);
   sgmse::g_inconv_variant = xl(o.inconv_variant, 2, 3);
@@ -1652,7 +1639,7 @@ static void activate(const sgmse_b200_engine& e) {
 extern "C" {
 
 const char* sgmse_b200_last_error(void) { return sgmse::get_last_error(); }
-const char* sgmse_b200_version(void) { return "sgmse_b200 0.1 (sm_100a)"; }
+const char* sgmse_b200_version(void) { return "sgmse_b200 0.1 (sm_90a)"; }
 
 int sgmse_b200_create(const sgmse_b200_config* cfg, sgmse_b200_engine** out) {
   API_BEGIN
@@ -1951,38 +1938,19 @@ int sgmse_b200_set_option(sgmse_b200_engine* e, const char* key, long long value
   }
   else if (k == "tc_variant") {
     // changes which intermediate buffers a forward needs: drop cached workspace sizes, graphs and shadow lanes
-    // 2, 3, 5 = the superseded kernel generations conv_tc2 / conv_tc3 / conv_tc5: compiled into the lab twin only
-    // 9, 10 = the TMA-fed in-place producer forms of conv_tc6 (fused modes 2 / 3): lab twin only as well
-    SG_CHECK((value != 2 && value != 3 && value != 5 && value != 9 && value != 10) || sgmse::lab_compiled(),
-             "tc_variant %lld selects a superseded kernel generation that exists in the lab twin library only "
-             "(python -m sgmse_b200.build --pdl, SGMSE_B200_PDL=1)", value);
+    SG_CHECK(value == 0 || value == 5, "tc_variant %lld: 0 (TMA-fed convolutions, separate GroupNorm passes) or 5 (GroupNorm+SiLU fused into the convolutions)", value);
     e->opts.tc_variant = (int)value;
     if (e->lanes.size() > 1) ensure_lanes(*e, 1);
     e->arena_need.clear();
     clear_graphs(*e);
   }
   else if (k == "attn_variant") { e->opts.attn_variant = (int)value; clear_graphs(*e); }
-  else if (k == "tc6_rings") { e->opts.tc6_rings = (int)value; clear_graphs(*e); }
-  else if (k == "tc6_mma") { e->opts.tc6_mma = (int)value; clear_graphs(*e); }
-  else if (k == "tc6_tma_poll") { e->opts.tc6_tma_poll = (int)value; clear_graphs(*e); }
-  else if (k == "tc6_roles") { e->opts.tc6_roles = (int)value; clear_graphs(*e); }
-  else if (k == "tc6_lean") {
-    SG_CHECK((value != 1 && value != 4) || sgmse::lab_compiled(),
-             "tc6_lean %lld selects a superseded producer form that exists in the lab twin library only", value);
-    e->opts.tc6_lean = (int)value;
-    clear_graphs(*e);
-  }
   else if (k == "fir_variant") { e->opts.fir_variant = (int)value; clear_graphs(*e); }
   else if (k == "inconv_variant") { e->opts.inconv_variant = (int)value; clear_graphs(*e); }
   else if (k == "combine_variant") { e->opts.combine_variant = (int)value; clear_graphs(*e); }
   else if (k == "tc1_narrow") { e->opts.tc1_narrow = (int)value; clear_graphs(*e); }
   else if (k == "gn_self") { e->opts.gn_self = (int)value; clear_graphs(*e); }
   else if (k == "gnfin_variant") { e->opts.gnfin_variant = (int)value; clear_graphs(*e); }
-  else if (k == "tc6_ablate") {
-    SG_CHECK(value == 0 || sgmse::lab_compiled(), "option 'tc6_ablate' exists in the lab twin library only");
-    e->opts.tc6_ablate = (int)value;
-    clear_graphs(*e);
-  }
   else if (k == "outconv_variant") {
     e->opts.outconv_variant = (int)value;       // changes the buffers a forward needs (fused GroupNorm or not)
     if (e->lanes.size() > 1) ensure_lanes(*e, 1);
@@ -2022,7 +1990,6 @@ long long sgmse_b200_get_counter(const sgmse_b200_engine* e, const char* key) {
   if (k == "graph_launches") return e->graph_launches;
   if (k == "cached_graphs") return (long long)e->graphs.size();
   if (k == "pdl_compiled") return sgmse::pdl_compiled() ? 1 : 0;
-  if (k == "lab_compiled") return sgmse::lab_compiled() ? 1 : 0;
   if (k == "pdl") return e->opts.pdl;
   if (k == "workspace_bytes") return (long long)e->arena.cap;
   if (k == "weights_bytes") return (long long)e->weights_bytes;

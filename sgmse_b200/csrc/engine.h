@@ -156,7 +156,7 @@ struct sgmse_b200_engine {
   // launch sequences on forked streams, so that the HBM-bound kernels of one lane (GroupNorm apply, FIR, PC
   // update) overlap the tensor-bound convolutions of the other.  A lane is a shadow engine: it shares the
   // packed weights (owns_weights == false) and owns its workspace, state and staging buffers.
-  int num_lanes = 1;                          // round 2: one lane is faster under the power cap (profiles/r02_step_trace.txt: 1 158 vs 1 189 ms per step)
+  int num_lanes = 1;                          // concurrent launch sequences inside a captured sampler graph (option "lanes")
   bool owns_weights = true;
   std::vector<sgmse_b200_engine*> lanes;      // lanes[0] == this
   std::vector<cudaStream_t> lane_streams;     // lane_streams[0] unused (lane 0 runs on the caller's stream)
@@ -168,7 +168,7 @@ struct sgmse_b200_engine {
   // point installs the calling engine's set first (engine.cu: activate), so two engines of one process -- or of two host
   // threads -- never see each other's choices, and a captured graph keeps the choices of the engine that captured it.
   struct KernelOpts {
-    int tc_variant = 0, tc1_narrow = 0, tc6_rings = 0, tc6_mma = 0, tc6_tma_poll = 0, tc6_roles = 0, tc6_lean = 0, tc6_ablate = 0;
+    int tc_variant = 0, tc1_narrow = 0;
     int attn_variant = 0, fir_variant = 0, inconv_variant = 0, outconv_variant = 0, combine_variant = 0;
     int gn_self = 0, gnfin_variant = 0, pdl = 0;
   } opts;

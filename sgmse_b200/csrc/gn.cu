@@ -13,16 +13,16 @@ namespace sgmse {
 // ------------------------------------------------------------------------------------------------
 // gn_finalize: grid (groups, N).  Sums the producer's per-slot partials in double, fixed order.
 // ------------------------------------------------------------------------------------------------
-// BATCH (gnfin_variant 1; round 2, the default since -- gated on a B200, bit-identical): the partials of a thread are loaded eight at a time before
+// BATCH (gnfin_variant 1; round 2, the default since -- bit-identical): the partials of a thread are loaded eight at a time before
 // they are added, in the same order (the plain loop is load -> add -> branch: 8 serialized round trips per thread at the 512-slot
-// levels, most of the kernel's 5.9 us); bit-identical.
+// levels, most of the kernel's time); bit-identical.
 thread_local int g_gnfin_variant = 0;
 
 template <bool BATCH>
 __global__ void gn_finalize_kernel(const float* __restrict__ st0, int C0, int slots0,
                                    const float* __restrict__ st1, int C1, int slots1,
                                    const float* __restrict__ gamma, const float* __restrict__ beta,
-                                   int cpg, double inv_count, float2* __restrict__ ab, uint4* __restrict__ ab16,
+                                   int cpg, double inv_count, float2* __restrict__ ab,
                                    unsigned int* __restrict__ range_flag) {
   pdl_trigger(); pdl_wait();
   const int g = blockIdx.x, n = blockIdx.y;
@@ -97,44 +97,26 @@ __global__ void gn_finalize_kernel(const float* __restrict__ st0, int C0, int sl
     const float a = gamma[ch] * rstd;
     ab[(size_t)n * Ct + ch] = make_float2(a, beta[ch] - (float)mean * a);
   }
-  // half2 form for the in-conv producers (conv_tc6 fused mode 3): per channel PAIR {m_hi, m_lo, a/2, beta/2} with
-  // mean = m_hi + m_lo split in two halfs, so that z/2 = (a/2) * ((x - m_hi) - m_lo) + beta/2 has no cancellation
-  // against a rounded constant.  cpg is even whenever this table is requested.
-  if (ab16)
-    for (int pl = threadIdx.x; pl < cpg / 2; pl += blockDim.x) {
-      const int ch = g * cpg + 2 * pl;
-      const float mf = (float)mean;
-      const __half mh = __float2half_rn(mf);
-      const __half ml = __float2half_rn(mf - __half2float(mh));
-      const __half2 m_hi = __halves2half2(mh, mh), m_lo = __halves2half2(ml, ml);
-      const __half2 ah = __floats2half2_rn(0.5f * gamma[ch] * rstd, 0.5f * gamma[ch + 1] * rstd);
-      const __half2 bh = __floats2half2_rn(0.5f * beta[ch], 0.5f * beta[ch + 1]);
-      uint4 v;
-      v.x = *reinterpret_cast<const uint32_t*>(&m_hi); v.y = *reinterpret_cast<const uint32_t*>(&m_lo);
-      v.z = *reinterpret_cast<const uint32_t*>(&ah); v.w = *reinterpret_cast<const uint32_t*>(&bh);
-      ab16[((size_t)n * Ct + ch) >> 1] = v;
-    }
 }
 
 void launch_gn_finalize(cudaStream_t st, const TensorDesc& s0, const TensorDesc* s1, const float* gamma,
-                        const float* beta, int groups, float2* ab, uint4* ab16, unsigned int* range_flag) {
+                        const float* beta, int groups, float2* ab, unsigned int* range_flag) {
   const int C1 = s1 ? s1->C : 0;
   const int Ct = s0.C + C1;
   SG_CHECK(Ct % groups == 0, "GroupNorm: %d channels not divisible by %d groups", Ct, groups);
   SG_CHECK(s0.stats && s0.slots > 0 && (!s1 || (s1->stats && s1->slots > 0)), "GroupNorm input has no statistics");
   if (s1) SG_CHECK(s1->N == s0.N && s1->H == s0.H && s1->W == s0.W, "concat shape mismatch");
   const int cpg = Ct / groups;
-  SG_CHECK(!ab16 || cpg % 2 == 0, "GroupNorm: the half2 coefficient table needs an even number of channels per group");
   const double inv_count = 1.0 / ((double)s0.H * s0.W * cpg);
   dim3 grid(groups, s0.N);
   if (g_gnfin_variant == 1) {
     launch_k(gn_finalize_kernel<true>, grid, dim3(256), 0, st, s0.stats, s0.C, s0.slots, s1 ? s1->stats : nullptr, C1,
-             s1 ? s1->slots : 0, gamma, beta, cpg, inv_count, ab, ab16, range_flag);
+             s1 ? s1->slots : 0, gamma, beta, cpg, inv_count, ab, range_flag);
     CUDA_OK(cudaGetLastError());
     return;
   }
   launch_k(gn_finalize_kernel<false>, grid, dim3(256), 0, st, s0.stats, s0.C, s0.slots, s1 ? s1->stats : nullptr, C1,
-                                           s1 ? s1->slots : 0, gamma, beta, cpg, inv_count, ab, ab16, range_flag);
+                                           s1 ? s1->slots : 0, gamma, beta, cpg, inv_count, ab, range_flag);
   CUDA_OK(cudaGetLastError());
 }
 
@@ -229,9 +211,9 @@ gn_apply_plain_kernel(const T* __restrict__ x0, int C0, const T* __restrict__ x1
 }
 
 // ------------------------------------------------------------------------------------------------
-// gn_self (round 2, on by default since -- gated on a B200, bit-identical): gn_finalize folded into the gn_apply_plain that
-// consumes it, for the small tensors of the levels below 32 rows (H*W <= 512), where a forward spends ~46 launches of
-// ~6 us on finalizing statistics that fit in a few hundred bytes.  Every block first rebuilds (a, b) of ITS sample in
+// gn_self (round 2, on by default since -- bit-identical): gn_finalize folded into the gn_apply_plain that
+// consumes it, for the small tensors of the levels below 32 rows (H*W <= 512), where a forward spends ~46 launches
+// on finalizing statistics that fit in a few hundred bytes.  Every block first rebuilds (a, b) of ITS sample in
 // shared memory -- warp w reduces groups w, w+8, ...: lane j adds the group's (channel, slot) items j, j+32, ... in
 // double and the warp combines them with the same xor tree gn_finalize uses, so for channels-per-group x slots <= 32
 // (one item per lane) the coefficients are bit-identical by construction; beyond that (a Combine output has 16 slots of 32
@@ -409,7 +391,7 @@ gn_apply_fir_kernel(const T* __restrict__ x0, int C, const float2* __restrict__ 
 // phase 2 applies the separable [1,3,3,1] FIR from smem and writes both outputs with 128-bit stores.
 // ------------------------------------------------------------------------------------------------
 thread_local int g_fir_variant = 0;   // 0: one-MUFU silu (tanh form) + half2 FIR-down arithmetic; 1: expf/divide silu, fp32 FIR;
-                         // 2 (round 2, the default since -- gated on a B200: FIR-down bit-identical, half2 FIR-up rel-L2 8e-4): 0 + all global loads of phase 1 in flight at once
+                         // 2 (round 2, the default since: FIR-down bit-identical, half2 FIR-up rel-L2 8e-4): 0 + all global loads of phase 1 in flight at once
                          //    (the SASS of 0 has ONE LDG.128 per loop trip in front of 8 MUFU: 4-6 serialized memory
                          //    round trips per thread) + half2 FIR-up over 2x2 output quads (9 instead of 16 LDS.128 and
                          //    ~50 instead of ~150 instructions per output vector)

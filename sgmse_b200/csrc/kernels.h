@@ -24,10 +24,8 @@ struct TensorDesc {
 
 // ---- GroupNorm ----
 // ab[n][c] = (a, b) with y = a*x + b  (a = gamma*rstd, b = beta - mean*rstd*gamma), eps = 1e-6
-// ab16 (optional): [n][Ct/2] per channel pair {half2 m_hi, half2 m_lo, half2 a/2, half2 beta/2}, mean = m_hi + m_lo
 void launch_gn_finalize(cudaStream_t st, const TensorDesc& s0, const TensorDesc* s1, const float* gamma,
-                        const float* beta, int groups, float2* ab, uint4* ab16 = nullptr,
-                        unsigned int* range_flag = nullptr);   // += 1 per (sample, group) whose fp16 input overflowed (non-finite sums)
+                        const float* beta, int groups, float2* ab, unsigned int* range_flag = nullptr);   // += 1 per (sample, group) whose fp16 input overflowed (non-finite sums)
 // stand-alone per-(sample, channel) statistics (slots = 1) for levels too small for per-tile partials
 void launch_channel_stats(cudaStream_t st, TensorDesc& t);
 enum Resample { RS_NONE = 0, RS_DOWN = 1, RS_UP = 2 };
@@ -61,10 +59,9 @@ struct ConvArgs {
   int temb_stride = 0;             // floats between consecutive samples' rows (0: all samples share)
   const TensorDesc* residual = nullptr;
   float scale = 1.f;               // out = (acc + bias + temb + residual) * scale
-  // Fused GroupNorm-apply + SiLU (conv_tc5 only): seg[0] (3x3) reads RAW tensors -- seg[0].src, concatenated with
+  // Fused GroupNorm-apply + SiLU (conv_tc only): seg[0] (3x3) reads RAW tensors -- seg[0].src, concatenated with
   // gn_cat when gn_has_cat -- and applies silu(a*x+b) with (a, b) = gn_ab[n][channel] on the way into shared memory.
   const float2* gn_ab = nullptr;
-  const uint4* gn_ab16 = nullptr;  // the same coefficients in the half2 form of launch_gn_finalize (conv_tc6 mode 3)
   bool gn_has_cat = false;
   TensorDesc gn_cat;
   int ktot() const {
@@ -74,35 +71,14 @@ struct ConvArgs {
   }
 };
 void launch_conv_direct(cudaStream_t st, const ConvArgs& a, TensorDesc& out);
-// tcgen05 implicit GEMM; requires fp16 activations, every segment C % 64 == 0, Cout % 128 == 0
+// wgmma implicit GEMM (conv_tc.cu); requires fp16 activations, every segment C % 64 == 0, Cout % 64 == 0
 bool conv_tc_supported(const ConvArgs& a, const TensorDesc& out);
+// shape test of the fused GroupNorm-apply/SiLU form (3x3 over c0 [+ c1] raw channels), usable before the tensors exist
+bool conv_tc_fuse_shape_ok(int H, int W, int c0, int c1, int cout);
 void launch_conv_tc(cudaStream_t st, const ConvArgs& a, TensorDesc& out, int* dbg_flag);
-// second-generation kernel (conv_tc2.cu): activation/weight tiles reused across taps and sub-tiles in smem;
-// needs W % 8 == 0, H % 16 == 0, Cout % 128 == 0.  launch_conv_tc dispatches to it unless g_tc_variant == 1.
-bool conv_tc2_supported(const ConvArgs& a, const TensorDesc& out);
-void launch_conv_tc2(cudaStream_t st, const ConvArgs& a, TensorDesc& out, int* dbg_flag);
-// third generation (conv_tc3.cu): CTA pairs, cta_group::2 M256 UMMAs; needs W % 16 == 0, H % 32 == 0 on top of v2.
-bool conv_tc3_supported(const ConvArgs& a, const TensorDesc& out);
-void launch_conv_tc3(cudaStream_t st, const ConvArgs& a, TensorDesc& out, int* dbg_flag);
-// fourth generation (conv_tc4.cu): operands swapped (channels = UMMA M, pixels = UMMA N = 256), half the MMA issues
-bool conv_tc4_supported(const ConvArgs& a, const TensorDesc& out);
-void launch_conv_tc4(cudaStream_t st, const ConvArgs& a, TensorDesc& out, int* dbg_flag);
-// fifth generation (conv_tc5.cu): v4 + GroupNorm-apply/SiLU of the 3x3 input fused into a software operand producer
-bool conv_tc5_shape_ok(int H, int W, int c0, int c1, int cout, int nraw);
-void launch_conv_tc5(cudaStream_t st, const ConvArgs& a, TensorDesc& out, int* dbg_flag);
-// sixth generation (conv_tc6.cu): one [34][10]-pixel halo tile per chunk, nine taps through shifted descriptors; optional
-// fused GroupNorm-apply/SiLU producer that evaluates each activation once
-bool conv_tc6_supported(const ConvArgs& a, const TensorDesc& out);
-bool conv_tc6_fuse_shape_ok(int H, int W, int c0, int c1, int cout, int nraw);
-void launch_conv_tc6(cudaStream_t st, const ConvArgs& a, TensorDesc& out, int* dbg_flag);
-extern thread_local int g_tc6_ablate;   // timing ablations of conv_tc6, compiled into the -DSGMSE_B200_PDL twin only (results are wrong on purpose)
-extern thread_local int g_tc6_rings, g_tc6_mma_style, g_tc6_tma_poll, g_tc6_roles, g_tc6_lean;   // conv_tc6 A/B switches, see conv_tc6.cu
-extern thread_local int g_tc1_narrow;   // 1: conv_tc v1 takes 64-wide channel tiles when 128-wide ones fill less than half the SMs (round 2, the default since)
-extern thread_local int g_tc_variant;   // 0 (= 7, 8): newest applicable kernels (v6 with fused GroupNorm+SiLU where possible: LDG-fed producers,
-                           // fp32 math = fused mode 1; else v4/v1), 1: v1 only, 2: v2 (+v1), 3: v3 CTA pairs (+v2, v1),
-                           // 4: v4 (+v1) without GroupNorm fusion, 5: v5 fused GN (+v4), 6: v6 without fusion (+v4),
-                           // 9: v6 fused, TMA-fed raw tile transformed in place, fp32 math (mode 2),
-                           // 10: the same with half2 math on the split-mean coefficient table (mode 3)
+extern thread_local int g_tc1_narrow;   // 1: 64-wide channel tiles when 128-wide ones fill less than half the SMs (the default)
+extern thread_local int g_tc_variant;   // 0: TMA-fed convolutions, separate gn_apply launches; 5: GroupNorm+SiLU fused into the 3x3
+                                        // convolutions where the shape allows (its producer re-evaluates every tap: 3.2x slower per benchmark step on H100)
 
 // input layer: state float4 (x.re,x.im,y.re,y.im) -> conv3x3(4->C); w [36][C] (k = tap*4+cin), bias [C]
 // in_scale multiplies the state on the way in (c_in of the preconditioned 'ncsnpp_v2' forward, model.py:284,312-319)
@@ -121,17 +97,15 @@ bool out_conv_fuses_gn(const TensorDesc& act);
 void launch_out_conv(cudaStream_t st, const TensorDesc& act, const float* w, const float* bias,
                      const float4* addend, float4* out, const float2* gn_ab = nullptr, const uint2* wfrag = nullptr);
 extern thread_local int g_outconv_variant;   // 0: mma.sync kernel for fp16 C in {128, 256}; 1: CUDA-core kernels; 2: mma.sync kernel with
-                                // GroupNorm+SiLU fused into its staging (measured slower than gn_apply + conv: profiles/)
+                                // GroupNorm+SiLU fused into its staging
                                 // 3: the mma.sync kernel with its tile staged by cp.async (round 2, the default since; see small.cu)
 extern thread_local int g_combine_variant;   // 0: thread per channel (2-byte accesses); 1: thread per 8-channel vector (round 2, the default since; bit-identical)
 extern thread_local int g_inconv_variant;    // 0: mma.sync input conv for fp16 C in {32, 64, 128}; 1: CUDA-core kernel; 2: 0 with prefetched A fragments (round 2, the default since)
 
 // ---- attention: qkv [N,H,W,3C] (q|k|v), out [N,H,W,C] = softmax(q k^T / sqrt(C)) v over H*W tokens
 void launch_attention(cudaStream_t st, const TensorDesc& qkv, TensorDesc& out);
-extern thread_local int g_attn_variant;   // 0: tcgen05 kernel (attn_umma.cu) where it applies, else the fp16 mma.sync flash kernel (C in {128,256}); 1: fp32 CUDA-core kernel; 2: mma.sync with cp.async tile staging; 3: mma.sync (the round-1 default)
-// tcgen05 attention (attn_umma.cu): fp16, C = 256, token count a multiple of 128 up to 512; TMA-staged Q/K/V, scores in TMEM
-bool attention_umma_supported(const TensorDesc& qkv, const TensorDesc& out);
-void launch_attention_umma(cudaStream_t st, const TensorDesc& qkv, TensorDesc& out, int* dbg = nullptr);
+extern thread_local int g_attn_variant;   // 0 (= 2): fp16 mma.sync flash kernel with cp.async tile staging (C in {128,256}); 1: fp32 CUDA-core
+                                          // kernel; 3: the mma.sync kernel with plain (LDG/STS) tile staging
 
 // ---- time embedding ----
 struct TembWeights {
@@ -198,7 +172,7 @@ void launch_langevin_coef(cudaStream_t st, const float4* pyr, int N, int H, int 
 // ---- probability-flow ODE sampler (SURVEY.md §8f-4; ode.cu, controller in rk45.h) ----
 struct OdeK { const float2* k[7]; };   // stage derivatives K_0..K_6, complex64 like the reference's drift_fn output
 struct OdeCoefs { double a[7]; };
-constexpr int kOdeNormBlocks = 592;    // 4 x 148 SMs; one fp64 partial per block, summed on the host in block order
+constexpr int kOdeNormBlocks = 528;    // 4 x 132 SMs; one fp64 partial per block, summed on the host in block order
 // stage = (complex64)(y + (sum_{j<s} a_j K_j) * h); y_new (nullable) receives the fp64 value
 void launch_ode_combine(cudaStream_t st, const double2* y, const OdeK& K, int s, const OdeCoefs& c, double h, size_t total,
                         float2* stage, double2* y_new);

@@ -16,13 +16,6 @@ bool pdl_compiled() {
   return false;
 #endif
 }
-bool lab_compiled() {                       // timing ablations + superseded convolution generations (build.py --pdl = the lab twin)
-#ifdef SGMSE_B200_LAB
-  return true;
-#else
-  return false;
-#endif
-}
 
 // ================================================================================================
 // time embedding

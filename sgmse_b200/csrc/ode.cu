@@ -132,7 +132,7 @@ static unsigned grid_for(size_t total, unsigned cap) {
 
 void launch_ode_combine(cudaStream_t st, const double2* y, const OdeK& K, int s, const OdeCoefs& c, double h, size_t total,
                         float2* stage, double2* y_new) {
-  ode_combine_kernel<<<grid_for(total, 148 * 16), 256, 0, st>>>(y, K, s, c, h, total, stage, y_new);
+  ode_combine_kernel<<<grid_for(total, 132 * 16), 256, 0, st>>>(y, K, s, c, h, total, stage, y_new);
   CUDA_OK(cudaGetLastError());
 }
 void launch_ode_drift(cudaStream_t st, const float4* state, const float4* pyr, int N, int H, int W, const OutLayer& ol,

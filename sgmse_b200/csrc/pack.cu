@@ -7,7 +7,7 @@
 
 namespace sgmse {
 
-// [k][cout] (fp32 or fp16) and, optionally, [cout][ld] fp16 (K-major, tcgen05) of up to four K segments.
+// [k][cout] (fp32 or fp16) and, optionally, [cout][ld] fp16 (K-major, conv_tc) of up to four K segments.
 //   mode 0: Conv2d weights [cout][cin][taps];  mode 1: NIN weights [cin][cout];
 //   mode 2: three NIN weights [cin][cout/3] side by side (q | k | v of the attention block; seg[0..2].w hold the three offsets)
 template <typename T>

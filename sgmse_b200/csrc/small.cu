@@ -69,14 +69,14 @@ __global__ void __launch_bounds__(128) input_conv_kernel(const float4* __restric
 
 // fp16 tensor-core variant (mma.sync m16n8k16): the 36-deep contraction (9 taps x 4 state components) is padded to
 // K = 48 = 3 k-steps; a warp owns 32 pixels x all C output channels (2 m-tiles x NT n-tiles).  The CUDA-core kernel
-// above needs 36 FMA per output element (FMA-bound: ~150 us for [16,256,512] -> 128 channels at full FP32 rate);
+// above needs 36 FMA per output element (FMA-bound);
 // here the arithmetic is 3 HMMA per 16x8 outputs and the kernel is bound by the 256 B/pixel it writes.
 //   A fragment (pixels x k): k = tap*4 + component, so the k pair (2t, 2t+1) of k-step s is the (.xy | .zw) half of the
 //   state float4 of neighbour tap 4s + (t >> 1) [a0/a1] and 4s + 2 + (t >> 1) [a2/a3]: straight from global/L1.
 //   B fragments (k x channels) are built once per block in shared memory; the block then walks tiles of 128 pixels.
 //   Output goes through a per-warp padded smem tile so that global stores are 128-bit and row-contiguous.
 thread_local int g_inconv_variant = 0;   // 0: tensor-core kernel for fp16 output where it applies, 1: CUDA-core kernel,
-                            // 2 (round 2, the default since -- gated on a B200, bit-identical): 0 with the A fragments of the NEXT 16-pixel m-tile
+                            // 2 (round 2, the default since -- bit-identical): 0 with the A fragments of the NEXT 16-pixel m-tile
                             //   loaded before the 48 MMAs of the current one (today every m-tile starts with an exposed
                             //   L1/L2 round trip at 16 warps per SM); same arithmetic, bit-identical
 
@@ -339,7 +339,7 @@ static void input_conv_mma_launch(cudaStream_t st, const float4* state, int N, i
   const size_t smem = (size_t)3 * NT * 32 * sizeof(uint2) + (size_t)4 * 32 * (C + 8) * 2 + (size_t)4 * C * 2 * 4;
   auto k = PREFETCH ? input_conv_mma_pf_kernel<NT, true> : input_conv_mma_kernel<NT>;
   CUDA_OK(cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-  const int grid = std::min(num_tiles, 148 * 4);
+  const int grid = std::min(num_tiles, 132 * 4);
   launch_k(k, dim3(grid), dim3(128), smem, st, state, H, W, w, bias, (__half*)out.p, out.stats, out.slots, num_tiles, in_scale);
   CUDA_OK(cudaGetLastError());
 }
@@ -403,10 +403,10 @@ __global__ void __launch_bounds__(128) combine_kernel(const float4* __restrict__
   }
 }
 
-// combine_variant 1 (round 2, the default since -- gated on a B200, bit-identical): a thread owns 8 channels (one 128-bit vector) of one
+// combine_variant 1 (round 2, the default since -- bit-identical): a thread owns 8 channels (one 128-bit vector) of one
 // 32-pixel tile and walks the tile's pixels in order -- the same per-channel expression and the same summation order as
 // the kernel above, so results and statistics are bit-identical -- with 8 vector loads in flight per thread instead of
-// four 2-byte ones (the scalar kernel keeps ~16 KB in flight per SM: 2.4 TB/s on the 268 MB of the top level).
+// four 2-byte ones (the scalar kernel keeps too few bytes in flight per SM to reach HBM bandwidth).
 thread_local int g_combine_variant = 0;
 
 template <int CV>   // CV = C / 8 vectors per pixel (16 or 32); block = 128 threads = 128 / CV tiles
@@ -634,10 +634,10 @@ __global__ void __launch_bounds__(256) out_conv_coop_kernel(const T* __restrict_
 // fp16 tensor-core variant (mma.sync m16n8k16, N = 8 with the 4 real outputs in columns 0..3): a block stages a
 // 16x16 pixel tile (+1 halo) of the activation in shared memory once, every warp computes two 16-pixel rows with
 // 9 taps x C/16 MMAs each.  ~15x fewer instructions than the CUDA-core kernels above; HBM/L2-bound.
-// ASYNC (outconv_variant 3; round 2, the default since -- gated on a B200, bit-identical): the 18x18-pixel tile is staged with cp.async
+// ASYNC (outconv_variant 3; round 2, the default since -- bit-identical): the 18x18-pixel tile is staged with cp.async
 // (16 B each, zero-filled outside the image), i.e. all ~20 (C = 128) / ~40 (C = 256) loads of a thread are in flight at
 // once.  The SASS of the plain staging loop is LDG.128 -> STS.128 -> branch: one memory round trip per loop trip, which
-// is why the kernel sits at 2.1 TB/s (260 us for 545 MB).  Same bytes in shared memory, same arithmetic: bit-identical.
+// is why the plain form stays well below HBM bandwidth.  Same bytes in shared memory, same arithmetic: bit-identical.
 template <int C, bool ASYNC = false>
 __global__ void __launch_bounds__(256) out_conv_mma_kernel(const __half* __restrict__ act, int H, int W,
                                                            const float* __restrict__ w, float4 bias,

@@ -1,7 +1,7 @@
 /* Plain-C client of the PRODUCT path: host waveforms in, enhanced host waveforms out, through sgmse_b200_enhance with
- * host_buffers = 1 -- the client calls no CUDA API itself.  Small NCSN++ (nf 64, 3 levels, F = 64), fp16 tcgen05 mode,
+ * host_buffers = 1 -- the client calls no CUDA API itself.  Small NCSN++ (nf 64, 3 levels, F = 64), fp16 wgmma mode,
  * pseudo-random weights, N = 2 predictor-corrector steps.  Checks: finite output, different from the input, bit-identical
- * for the same (seed, utterance id), different for another seed.  Needs a B200: run by the -m gpu test
+ * for the same (seed, utterance id), different for another seed.  Needs a GPU: run by the -m gpu test
  * tests/test_gpu_zz_next_rows.py::test_plain_c_client_on_the_product_path. */
 #include <math.h>
 #include <stdio.h>
@@ -78,7 +78,7 @@ int main(void) {
   }
   CHECK(memcmp(out1, out2, sizeof out1) == 0, "same (seed, utterance id) -> bit-identical");
   CHECK(diff > 0.0 && diff_seed > 0.0, "the sampler did something, the seed matters");
-  CHECK(sgmse_b200_get_counter(e, "tc_convs_last_forward") > 0, "tcgen05 convolutions ran");
+  CHECK(sgmse_b200_get_counter(e, "tc_convs_last_forward") > 0, "wgmma convolutions ran");
   CHECK(sgmse_b200_get_counter(e, "graph_launches") >= 2, "CUDA graph replay");
   printf("cabi_gpu ok: %lld parameters, mean |out - in| %.4f, kernels launched %lld\n", total, diff / (B * L),
          sgmse_b200_get_counter(e, "kernel_launches"));

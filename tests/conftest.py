@@ -9,7 +9,7 @@ if ROOT not in sys.path:
 
 
 def pytest_configure(config):
-    config.addinivalue_line("markers", "gpu: needs a CUDA device (run on the B200 box)")
+    config.addinivalue_line("markers", "gpu: needs a CUDA device (run on a GPU host)")
     config.addinivalue_line("markers", "slow: takes more than a few seconds on CPU")
 
 
@@ -27,7 +27,7 @@ def pytest_collection_modifyitems(config, items):
         has_gpu = False
     if has_gpu:
         return
-    skip = pytest.mark.skip(reason="needs a CUDA device (run on the B200 box: pytest -m gpu)")
+    skip = pytest.mark.skip(reason="needs a CUDA device (run on a GPU host: pytest -m gpu)")
     for item in items:
         if "gpu" in item.keywords:
             item.add_marker(skip)

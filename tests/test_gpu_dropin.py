@@ -1,12 +1,13 @@
 """The drop-in itself on hardware (SURVEY.md §8b, §8f-3): a live, UNMODIFIED reference ``ScoreModel`` (imported from the staged
 copy ``oracle/_ref`` -- see oracle/build_ref.py -- or from /root/reference where that exists), ``sgmse_b200.install(model)``,
 then the reference's own public calls: ``model.enhance(y)``, ``model.get_pc_sampler(...)()``, ``model(x_t, y, t)``
-(/root/reference/sgmse/model.py:264-310,348-368,426-465), compared with the same model before installation, run on the CPU
+(sgmse/model.py:264-310,348-368,426-465), compared with the same model before installation, run on the CPU
 with the same injected noise.  Second half: the in-training evaluation flow (model.py:205-257, util/inference.py:16-63):
 ``install(rebind_forward="no_grad", refresh_on_eval=True)``, weights change, the EMA swap of ``eval()`` -- reached the way
 Lightning + DDP reach it, through ``nn.Module.eval(wrapper)`` -- and ``enhance`` must follow the swapped-in weights.
 
-Run on the B200 box: ``pytest -m gpu``.  Skipped when neither /root/reference nor oracle/_ref is present.
+Run on a GPU host: ``pytest -m gpu``.  The reference package is imported from the copy that ``__graft_entry__.build()``
+stages under oracle/_ref (oracle/build_ref.py), or from a live checkout; skipped when neither is present.
 """
 import numpy as np
 import pytest
@@ -17,12 +18,12 @@ from oracle import refshim, sde as o_sde, pipeline as o_pipe
 pytestmark = [pytest.mark.gpu,
               pytest.mark.skipif(not refshim.reference_available(), reason="reference not staged (oracle/_ref) and no live checkout")]
 
-# mid-size config: 64..128 channels -> the tcgen05 convolutions run in fp16_tc mode (same as MID_E in test_gpu_parity.py)
+# mid-size config: 64..128 channels -> the wgmma convolutions run in fp16_tc mode (same as MID_E in test_gpu_parity.py)
 MID = dict(nf=64, ch_mult=(1, 2, 2), image_size=64, attn_resolutions=(16,), num_res_blocks=1, n_fft=126, hop_length=32)
 L, N = 4000, 3
 
-# measured on a B200 (profiles/r02_parity.txt): fp32 sampler 1.6e-6 / waveform 1.5e-6 / forward 3.3e-6; fp16_tc 1.30e-3 /
-# 1.08e-3 (SI-SDR 59.4 dB) / 2.66e-3; bounds = 2x measured
+# measured on an H100: fp32 sampler 1.6e-6 / waveform 1.4e-6 / forward 3.4e-6; fp16_tc 1.21e-3 /
+# 1.03e-3 (SI-SDR 59.7 dB) / 2.46e-3; bounds about 2x measured
 TOL = {"fp32": dict(spec=3.3e-6, wav=3e-6, fwd=6.7e-6), "fp16_tc": dict(spec=2.6e-3, wav=2.2e-3, fwd=5.4e-3)}
 
 
@@ -78,7 +79,7 @@ def test_install_on_a_live_reference_score_model(mode):
         with torch.no_grad():
             e_fwd = rel_l2(model(x_t.cuda(), Y.cuda(), t.cuda()), ref_score)
         if mode == "fp16_tc":
-            assert eng.counter("tc_convs_last_forward") > 0, "tcgen05 path not taken"
+            assert eng.counter("tc_convs_last_forward") > 0, "wgmma path not taken"
         print(f"drop-in {mode}: sampler rel-L2 {e_spec:.3e}, waveform rel-L2 {e_wav:.3e}, SI-SDR(ref, engine) {sdr:.1f} dB, "
               f"forward rel-L2 {e_fwd:.3e}")
         tol = TOL[mode]
@@ -161,7 +162,7 @@ def test_in_training_evaluation_follows_the_ema_swap():
         e = rel_l2(got_S, ref_S)
         print(f"in-training evaluation: after the EMA swap rel-L2 {e:.3e} vs the reference on the swapped weights "
               f"({rel_l2(got_S, ref_W):.3e} vs the training weights)")
-        assert e < 3e-6 and rel_l2(got_S, ref_W) > 5e-3                # measured 1.44e-6
+        assert e < 3e-6 and rel_l2(got_S, ref_W) > 5e-3                # measured 1.44e-6 on an H100
         # the validation loss route: _step -> self(x_t, y, t) under torch.no_grad() goes to the engine (EMA weights) ...
         with torch.no_grad():
             out = model(x_t.cuda(), Y.cuda(), t.cuda())

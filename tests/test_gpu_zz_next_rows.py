@@ -1,7 +1,5 @@
-"""GPU parity tests of the rows SURVEY.md §8(f) marks "next" that were written at the very end of round 1.  The
-small-config ODE tests and the batched-service test passed on a B200 in the round's last GPU call
-(profiles/r01_ode_first_contact.txt); the two full-size tests had no GPU minutes left.  The file name sorts after
-test_gpu_parity.py so that `pytest -x -m gpu` reports the core path first.  Run on the B200 box: ``pytest -m gpu``.
+"""GPU parity tests of the rows SURVEY.md §8(f) marks "next".  The file name sorts after
+test_gpu_parity.py so that `pytest -x -m gpu` reports the core path first.  Run on a GPU host: ``pytest -m gpu``.
 
 Tolerances: fp32 mode rel-L2 <= 1e-3 against the reference fixture after a full adaptive ODE solve; fp16_tc <= 3e-2.
 """
@@ -161,12 +159,9 @@ def test_full_size_prior_draw_statistics(full_sd):
     eng.close()
 
 
-# Bounds of the N = 30 run = twice the error measured on a B200 (profiles/r02_parity.txt): fp32 mode 91.6 dB / 2.66e-5;
-# product mode 34.2 dB / 1.97e-2.  The product-mode figure is the random walk of fp16 STORAGE rounding through 60 network
-# evaluations, not an arithmetic defect: mode fp16_direct (CUDA-core convolutions, exact expf SiLU, fp32 FIR -- nothing in
-# common with fp16_tc but the storage format) lands at 34.3 dB, the two fp16 pipelines are 48.8 dB from each other, and
-# single-approximation toggles move the figure by -3 .. +3 dB in either direction (tools/parity_decompose.py).  A CPU
-# emulation of fp16 storage on a 0.5-s clip had predicted 41 dB.
+# Bounds of the N = 30 run: about twice the error measured on an H100 (fp32 mode 91.6 dB / 2.66e-5; product mode 37.4 dB /
+# 1.35e-2), with room for the product-mode figure, which is the random walk of fp16 STORAGE rounding through 60 network
+# evaluations, not an arithmetic defect: single-approximation toggles move it by a few dB either way (tools/parity_decompose.py).
 FULL_N30_FP32_SDR, FULL_N30_FP32_REL = 85.6, 5.4e-5
 FULL_N30_TC_SDR, FULL_N30_TC_REL = 28.2, 4e-2
 
@@ -220,7 +215,7 @@ def test_full_size_v2_sb_ode_on_the_product_path(full_sd):
     got, n = eng.sb_sample(y.cuda(), sampler_type="ode", N=2)
     err = rel_l2(got, ref)
     print(f"full-size v2 SB-ODE (fp16_tc, edm preconditioning): rel-L2 {err:.3e}")
-    assert n == 50 and eng.counter("tc_convs_last_forward") > 0 and err < 4.4e-3           # measured 2.19e-3
+    assert n == 50 and eng.counter("tc_convs_last_forward") > 0 and err < 4.4e-3           # measured 2.09e-3 (H100)
     eng.close()
 
 
@@ -240,8 +235,8 @@ def test_full_size_ode_on_the_product_path(full_sd):
                                   return_stats=True)
     err = rel_l2(got, ref)
     print(f"full-size ODE (fp16_tc): nfe {nfe} (oracle {nfe_ref}), {st}, rel-L2 {err:.3e}")
-    # measured 1.1e-3 (round-1 kernels) and 4.1e-3 (round-2 defaults), nfe 32 = 32 both times: an adaptive solve at rtol 5e-2
-    # amplifies rounding-level differences between kernel variants through its step-size decisions
+    # measured 2.2e-3 on an H100, nfe 32 = 32: an adaptive solve at rtol 5e-2 amplifies rounding-level differences between
+    # kernel variants through its step-size decisions, hence the wider bound
     assert st["status"] == 0 and abs(nfe - nfe_ref) <= 12 and err < 8.3e-3
     assert eng.counter("tc_convs_last_forward") > 0
     eng.close()
@@ -363,7 +358,7 @@ def test_graph_cache_is_bounded(golden_dir):
 
 def test_plain_c_client_on_the_product_path(tmp_path):
     """tests/c/cabi_gpu.c: a C99 program (no Python, no C++, no CUDA call of its own) enhances two clips through
-    sgmse_b200_enhance with host buffers on the fp16 tcgen05 path and checks finiteness, seed determinism and graph replay."""
+    sgmse_b200_enhance with host buffers on the fp16 wgmma path and checks finiteness, seed determinism and graph replay."""
     import shutil
     import subprocess
     from sgmse_b200 import _lib, build
@@ -382,24 +377,19 @@ def test_plain_c_client_on_the_product_path(tmp_path):
     assert r.returncode == 0 and "cabi_gpu ok" in r.stdout, r.stdout + r.stderr
 
 
-# ---- the round-2 kernel candidates became the defaults (gated on a B200: profiles/r02_candidates_gate.txt); the round-1 kernels
+# ---- the round-2 kernel candidates became the defaults ; the round-1 kernels
 # stay selectable under a new option number and must still agree with the defaults ------------------------------------------
 # (option, number of the ROUND-1 kernel, tolerance against the current default = 0)
 CANDIDATES = [("outconv_variant", 4, 0.0), ("inconv_variant", 3, 0.0), ("attn_variant", 3, 2e-3), ("combine_variant", 2, 0.0),
-              ("tc1_narrow", 2, 0.0), ("gn_self", 2, 0.0), ("gnfin_variant", 2, 0.0), ("fir_variant", 3, 2e-3), ("tc6_lean", 4, 0.0),
-              ("tc6_lean", 1, 0.0)]
+              ("tc1_narrow", 2, 0.0), ("gn_self", 2, 0.0), ("gnfin_variant", 2, 0.0), ("fir_variant", 3, 2e-3)]
 
 
 @pytest.mark.parametrize("key,val,tol", CANDIDATES)
 def test_round1_kernels_agree_with_the_defaults(full_sd, key, val, tol):
     """Same arithmetic with different memory pipelining / tiling / thread mapping -> bit-identical network output (tol 0.0); the
-    half2 FIR-up of the default FIR kernel -> rel-L2 <= 2e-3 against the round-1 fp32 form (measured 8.3e-4); the tcgen05
-    attention kernel against the mma.sync one <= 1e-3."""
+    half2 FIR-up of the default FIR kernel -> rel-L2 <= 2e-3 against the round-1 fp32 form; the attention kernel with cp.async
+    tile staging (default) against its plain-staging form <= 2e-3."""
     eng = Engine(EngineConfig(mode="fp16_tc", max_batch=2, use_graphs=False))
-    if key == "tc6_lean" and eng.counter("lab_compiled") == 0:
-        eng.close()
-        pytest.skip("the superseded conv_tc6 producer forms are compiled into the lab twin only (SGMSE_B200_PDL=1); "
-                    "verified bit-identical on a B200 in round 2 (profiles/r02_parity.txt)")
     eng.load_state_dict(full_sd)
     g = torch.Generator().manual_seed(3)
     x = (torch.complex(torch.randn(2, 2, 256, 128, generator=g), torch.randn(2, 2, 256, 128, generator=g)) * 0.3).cuda()
@@ -422,7 +412,7 @@ def test_two_rank_nccl_shard_invariance():
     import subprocess
     import sys
     if torch.cuda.device_count() < 2:
-        pytest.skip("needs 2 GPUs (gpurun --gpus 2)")
+        pytest.skip("needs 2 GPUs")
     root = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
     r = subprocess.run([sys.executable, "-m", "torch.distributed.run", "--nnodes=1", "--nproc-per-node", "2", "--master-addr", "127.0.0.1",
                         "--master-port", "29533", os.path.join(root, "tools", "nccl_invariance.py")], capture_output=True, text=True, timeout=900)

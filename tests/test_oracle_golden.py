@@ -236,7 +236,7 @@ MID_PAIRS = [("reverse_diffusion", "ald", 3), ("reverse_diffusion", "langevin", 
 
 
 def test_mid_size_fixture_is_reproduced_by_the_oracle(golden_dir):
-    """tests/golden/ncsnpp_mid.npz (oracle/make_golden.py: golden_mid_tc): reference outputs on the tcgen05-tileable
+    """tests/golden/ncsnpp_mid.npz (oracle/make_golden.py: golden_mid_tc): reference outputs on the tensor-core-tileable
     mid-size config, weights from oracle/weights.py seed 5 -- the pin of the product-mode GPU tests."""
     from oracle import weights as o_w
     z = np.load(os.path.join(golden_dir, "ncsnpp_mid.npz"))

@@ -3,7 +3,7 @@
     python tools/ab_forward.py [--batch 16] [--reps 4] tc_variant=8 tc_variant=0 inconv_variant=1 ...
 
 Each positional `key=value` is applied on top of the defaults (all variants 0) for one measurement, then reset.
-Prints ms per forward (CUDA events around `reps` forwards) and the summed tcgen05 conv time of one forward.
+Prints ms per forward (CUDA events around `reps` forwards) and the summed wgmma conv time of one forward.
 """
 import argparse
 import os
@@ -30,8 +30,8 @@ F = cfg.n_fft // 2 + 1
 g = torch.Generator().manual_seed(0)
 x = (torch.complex(torch.randn(a.batch, 2, F, a.T, generator=g), torch.randn(a.batch, 2, F, a.T, generator=g)) * 0.3).cuda()
 t = torch.full((a.batch,), 0.5).cuda()
-DEFAULTS = {"tc_variant": 0, "inconv_variant": 0, "outconv_variant": 0, "fir_variant": 0, "attn_variant": 0, "combine_variant": 0, "tc1_narrow": 0, "gn_self": 0, "gnfin_variant": 0, "tc6_ablate": 0, "tc6_rings": 0, "tc6_mma": 0,
-            "tc6_tma_poll": 0, "tc6_roles": 0, "tc6_lean": 0, "pdl": 0}     # pdl=1 needs SGMSE_B200_PDL=1 (libsgmse_b200_pdl.so, `python -m sgmse_b200.build --pdl`)
+DEFAULTS = {"tc_variant": 0, "inconv_variant": 0, "outconv_variant": 0, "fir_variant": 0, "attn_variant": 0, "combine_variant": 0, "tc1_narrow": 0, "gn_self": 0, "gnfin_variant": 0,
+            "pdl": 0}     # pdl=1 needs SGMSE_B200_PDL=1 (libsgmse_b200_pdl.so, `python -m sgmse_b200.build --pdl`)
 settings = ["default"] + a.settings
 times = {k: [] for k in settings}
 convs = {}

@@ -1,12 +1,12 @@
-"""Round-2 A/B of programmatic dependent launch (PDL) -- written at the end of round 1; run in round 2: bit-identical, slower (profiles/r02_pdl_check.txt).
+"""A/B of programmatic dependent launch (PDL): correctness against the default library, then timing.
 
     python -m sgmse_b200.build --pdl                 # here (cross-compiles): sgmse_b200/lib/libsgmse_b200_pdl.so
-    SGMSE_B200_PDL=1 python tools/check_pdl.py       # on the B200 box: correctness first, then timing
+    SGMSE_B200_PDL=1 python tools/check_pdl.py       # on the GPU: correctness first, then timing
 
 The default library carries no PDL instruction (cuobjdump: 0 x ACQBULK / PREEXIT); the twin is the same sources with
 -DSGMSE_B200_PDL, and even there the launches stay plain until `set_option("pdl", 1)`.  With PDL every kernel of the
 launch sequence triggers its dependents at entry and waits (griddepcontrol.wait) after its on-chip prologue, so barrier
-initialisation, TMEM allocation, tensor-map prefetch and weight-fragment staging of kernel k+1 overlap the tail of
+initialisation, tensor-map prefetch and weight-fragment staging of kernel k+1 overlap the tail of
 kernel k -- inside the captured sampler graph as programmatic dependency edges.
 
 Checks (bitwise): sampler output with pdl=1 == pdl=0, eager and graph-replayed, small config (fp32 + fp16_tc) and the

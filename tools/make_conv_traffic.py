@@ -1,11 +1,11 @@
-"""profiles/r02_conv_traffic.json from an ncu metrics pass of the CURRENT build (run on the GPU box, same snapshot):
+"""profiles/r02_conv_traffic.json (read by bench.py) from an ncu metrics pass of the CURRENT build:
 
-    ncu --clock-control none -k regex:conv_tc6 -s 54 -c 1 --metrics dram__bytes_read.sum,dram__bytes_write.sum,gpu__time_duration.sum \\
-        --csv --log-file gpurun_out/conv_traffic.csv python tools/profile_forward.py --batch 16 --evals 2
-    python tools/make_conv_traffic.py gpurun_out/conv_traffic.csv > profiles/r02_conv_traffic.json
+    ncu --clock-control none -k regex:conv_tc_kernel -s 54 -c 1 --metrics dram__bytes_read.sum,dram__bytes_write.sum,gpu__time_duration.sum \\
+        --csv --log-file /tmp/conv_traffic.csv python tools/profile_forward.py --batch 16 --evals 2
+    python tools/make_conv_traffic.py /tmp/conv_traffic.csv > profiles/r02_conv_traffic.json
 
--s 54 skips the first forward's 54 conv_tc6 launches (cold), so the captured launch is the first conv_tc6 launch of the
-second forward = ResBlock m4 Conv_0, the dominant shape.  The file records a digest of the kernel's sources; bench.py reports
+-s N skips the first forward's N conv_tc launches (cold, N = tc_convs_last_forward of the profiled forward), so the captured
+launch is the first conv_tc launch of the second forward.  The file records a digest of the kernel's sources; bench.py reports
 `roofline.traffic` only while that digest matches the sources it is run with (a stale capture is reported as null)."""
 import csv
 import hashlib
@@ -14,7 +14,7 @@ import os
 import sys
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-KERNEL_SOURCES = ["sgmse_b200/csrc/conv_tc6.cu", "sgmse_b200/csrc/common.cuh"]    # the kernel and its device helpers (kernels.h holds declarations only)
+KERNEL_SOURCES = ["sgmse_b200/csrc/conv_tc.cu", "sgmse_b200/csrc/common.cuh"]    # the kernel and its device helpers (kernels.h holds declarations only)
 
 
 def source_digest():

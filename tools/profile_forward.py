@@ -1,6 +1,6 @@
 """Run a few eager (un-graphed) score-network evaluations at the benchmark shape, for ncu.
 
-    ncu --metrics gpu__time_duration.sum --clock-control none --csv --log-file gpurun_out/launches.csv \
+    ncu --metrics gpu__time_duration.sum --clock-control none --csv --log-file /tmp/launches.csv \
         python tools/profile_forward.py --batch 16 --evals 2
 """
 import argparse

@@ -4,9 +4,8 @@
 
 Builds the .cu files of <git-rev> into a scratch directory with the flags of sgmse_b200/build.py, dumps the SASS of
 every kernel of both builds, demangles and normalises the names (anonymous-namespace hashes; template parameters that
-were renamed are listed as missing/new) and reports which kernels have an identical instruction stream.  Used at the end
-of round 1, when A/B candidates (PDL twin library, fir_variant 2, outconv_variant 3, inconv_variant 2) were added without
-GPU minutes: the kernels of the default launch sequence had to stay instruction-for-instruction what the B200 had verified.
+were renamed are listed as missing/new) and reports which kernels have an identical instruction stream: a refactor that leaves the default kernels
+instruction-for-instruction unchanged needs no new GPU verification.
 """
 import difflib
 import glob

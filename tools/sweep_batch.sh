@@ -1,11 +1,11 @@
 #!/bin/bash
 # BASELINE.json configs[4]: batch sweep 1 -> 512 synthetic 4-s clips, N = 30, on G GPUs of one box (default 1).
-#   bash tools/sweep_batch.sh [G]        -> one bench.py JSON line per batch size in gpurun_out/sweep_g${G}.jsonl
+#   bash tools/sweep_batch.sh [G]        -> one bench.py JSON line per batch size in ${OUT:-sweep_out}/sweep_g${G}.jsonl
 # Per-GPU batch b is sampled in micro-batches of min(b, 16) (one captured graph per micro-batch shape); under
 # torch.distributed.run the same line shards G*b clips over G ranks with no data-path collective.
 G=${1:-1}
-mkdir -p gpurun_out
-out=gpurun_out/sweep_g${G}.jsonl
+mkdir -p "${OUT:-sweep_out}"
+out=${OUT:-sweep_out}/sweep_g${G}.jsonl
 : > $out
 for b in 1 2 4 8 16 32 64 128 256 512; do
   mb=$(( b < 16 ? b : 16 ))
