@@ -18,7 +18,7 @@ CSRC = os.path.join(HERE, "csrc")
 LIBDIR = os.path.join(HERE, "lib")
 LIBNAME = "libsgmse_b200.so"
 SOURCES = ["gn.cu", "conv_direct.cu", "conv_tc.cu", "small.cu", "attn.cu", "misc.cu", "pack.cu", "ode.cu", "engine.cu"]
-HEADERS = ["common.cuh", "kernels.h", "engine.h", "rk45.h", os.path.join("..", "..", "include", "sgmse_b200.h")]
+HEADERS = ["common.cuh", "kernels.h", "conv_tc_sched.h", "engine.h", "rk45.h", os.path.join("..", "..", "include", "sgmse_b200.h")]
 
 NVCC = os.environ.get("NVCC", "/usr/local/cuda/bin/nvcc")
 CUDA_LIB = os.environ.get("CUDA_LIB", "/usr/local/cuda/lib64")

@@ -254,6 +254,16 @@ __device__ __forceinline__ bool elect_one() {
 __device__ __forceinline__ void named_bar_sync(int id, int nthreads) {
   asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(nthreads) : "memory");
 }
+// signal a named barrier without waiting on it (the waiting side calls named_bar_sync with the same count)
+__device__ __forceinline__ void named_bar_arrive(int id, int nthreads) {
+  asm volatile("bar.arrive %0, %1;" ::"r"(id), "r"(nthreads) : "memory");
+}
+// Per-thread register budget of the calling warpgroup (all 128 threads execute it): dec returns registers to the CTA's
+// pool, inc blocks until the pool has enough.  N is a multiple of 8 in [24, 256].
+template <int N>
+__device__ __forceinline__ void setmaxnreg_dec() { asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(N)); }
+template <int N>
+__device__ __forceinline__ void setmaxnreg_inc() { asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(N)); }
 #endif  // __CUDACC__
 
 }  // namespace sgmse

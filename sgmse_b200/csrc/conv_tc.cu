@@ -10,15 +10,18 @@
 // K segments let one accumulator take  conv3x3(h) + conv1x1(x_a) + conv1x1(x_b)  (ResnetBlockBigGANpp's
 // Conv_1 plus the Conv_2 shortcut over a concatenated skip input) without materialising the concat.
 //
-// Persistent, warp-specialised CTA (384 threads = 3 warpgroups, 1 CTA/SM):
-//   warpgroup 0   producer: one thread issues the TMA loads into an smem ring of NUM_STAGES x {A 16 KB,
-//                 B BLOCK_N*128 B}.  With FUSED (GroupNorm-apply + SiLU of the 3x3 input, see below) all 128
-//                 threads build the segment-0 A tiles from the RAW tensor instead.
-//   warpgroups 1, 2   wgmma m64nBLOCK_Nk16 on rows [64 wg, 64 wg + 64) of the tile, then the epilogue straight from
-//                 the accumulator registers: +bias +time-embedding bias +residual, *scale -> fp16 -> swizzled smem
-//                 staging -> TMA store; per-channel (sum, sum^2) partials for the next GroupNorm are reduced from
-//                 the staged tile (deterministic, no atomics).  The producer runs ahead into the next tile's
-//                 stages while the epilogue drains.
+// Persistent, warp-specialised CTA (384 threads = 3 warpgroups, 1 CTA/SM), "ping-pong" consumers:
+//   warpgroup 0   producer (register budget cut with setmaxnreg): one thread issues the TMA loads into an smem ring
+//                 of NUM_STAGES x {A 16 KB, B BLOCK_N*128 B}, in tile order.  With FUSED (GroupNorm-apply + SiLU of
+//                 the 3x3 input, see below) all 128 threads build the segment-0 A tiles from the RAW tensor instead.
+//   warpgroups 1, 2   (register budget raised with setmaxnreg) each own every other tile of the CTA (local tiles
+//                 j & 1 == 0 and 1) and compute the whole 128-pixel tile: two wgmma m64nBLOCK_Nk16 per k16 step
+//                 (rows 0-63 and 64-127).  The MMA turn passes between them through a pair of named barriers once
+//                 per tile (conv_tc_sched.h), so one warpgroup's epilogue runs while the other's MMAs keep the
+//                 tensor cores busy.  The epilogue works straight from the accumulator registers: +bias
+//                 +time-embedding bias +residual, *scale -> fp16 -> the warpgroup's own swizzled smem staging ->
+//                 TMA store; per-channel (sum, sum^2) partials for the next GroupNorm are reduced from the staged
+//                 tile (deterministic, no atomics).
 //
 // FUSED: out = conv3x3(silu(a * x + b)) with (a, b) = gn_ab[n][channel] (launch_gn_finalize) over the raw input x
 // (seg[0].src, concatenated with gn_cat), so the gn_apply pass and its buffer disappear.  Out-of-image taps read 0
@@ -28,6 +31,7 @@
 // (layers.py:546-555); the epilogue fuses `h += Dense_0(act(temb))[:, :, None, None]`, the Conv_2
 // shortcut add and `(x + h) / sqrt(2)` (layerspp.py:262-274).
 #include "kernels.h"
+#include "conv_tc_sched.h"
 
 #include <mutex>
 
@@ -39,7 +43,6 @@ constexpr int BLOCK_M = 128;
 constexpr int BLOCK_K = 64;     // fp16 elements = 128 B = one swizzle row
 constexpr int WG_K = 16;
 constexpr int NUM_THREADS = 384;
-constexpr int NUM_CONS = 256;   // the two MMA/epilogue warpgroups
 constexpr int A_TILE_BYTES = BLOCK_M * BLOCK_K * 2;   // 16 KB
 
 struct TcParams {
@@ -71,13 +74,15 @@ struct SmemLayout {
   static constexpr int B_TILE_BYTES = BLOCK_N * BLOCK_K * 2;
   static constexpr int STAGE_BYTES = A_TILE_BYTES + B_TILE_BYTES;
   static constexpr int N_CHUNKS = BLOCK_N / 64;
-  static constexpr int STAGING_BYTES = N_CHUNKS * A_TILE_BYTES;
+  static constexpr int STAGING_BYTES = N_CHUNKS * A_TILE_BYTES;         // per consumer warpgroup
+  static constexpr int STATS_BYTES = 4 * BLOCK_N * 2 * 4;               // per consumer warpgroup: float [4][BLOCK_N][2]
   static constexpr int OFF_STAGING = NUM_STAGES * STAGE_BYTES;
-  static constexpr int OFF_STATS = OFF_STAGING + STAGING_BYTES;         // float [4][BLOCK_N][2]
-  static constexpr int OFF_BARS = OFF_STATS + 4 * BLOCK_N * 2 * 4;
-  static constexpr int NUM_BARS = 2 * NUM_STAGES + 1;
+  static constexpr int OFF_STATS = OFF_STAGING + 2 * STAGING_BYTES;
+  static constexpr int OFF_BARS = OFF_STATS + 2 * STATS_BYTES;
+  static constexpr int NUM_BARS = 2 * NUM_STAGES + 2;                   // full[], empty[], residual[2]
   static constexpr int TOTAL = OFF_BARS + NUM_BARS * 8;
   static constexpr int DYN_BYTES = TOTAL + 1024;                        // slack for 1024 B alignment
+  static_assert(DYN_BYTES <= 227 * 1024, "conv_tc: shared memory over the sm_90 per-block limit");
 };
 
 // wgmma shared-memory matrix descriptor: K-major, SWIZZLE_128B canonical layout (8-row x 128 B atoms, 1024 B apart)
@@ -154,6 +159,12 @@ __device__ __forceinline__ void fused_a_row(uint8_t* tile, int r, const TcParams
   }
 }
 
+// Register budgets (setmaxnreg) of the two roles; 128 producer + 256 consumer threads share the 384 x 168 registers the
+// CTA is launched with.  The FUSED producer runs fused_a_row on all its threads and needs more than the TMA issuer.
+template <bool FUSED> struct TcRegs;
+template <> struct TcRegs<false> { static constexpr int PRODUCER = 40, CONSUMER = 232; };
+template <> struct TcRegs<true> { static constexpr int PRODUCER = 56, CONSUMER = 224; };
+
 template <int BLOCK_N, int NUM_STAGES, bool FUSED>
 __global__ void __launch_bounds__(NUM_THREADS, 1)
 conv_tc_kernel(const __grid_constant__ CUtensorMap map_a0, const __grid_constant__ CUtensorMap map_a1,
@@ -161,21 +172,21 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap map_a0, const __grid_constant
                const __grid_constant__ CUtensorMap map_d, const __grid_constant__ CUtensorMap map_r,
                const TcParams P) {
   using L = SmemLayout<BLOCK_N, NUM_STAGES>;
+  using R = TcRegs<FUSED>;
+  static_assert(128 * R::PRODUCER + 256 * R::CONSUMER <= NUM_THREADS * 168, "conv_tc: register budgets over the CTA's");
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023);
 
   uint64_t* bars = reinterpret_cast<uint64_t*>(smem + L::OFF_BARS);
   uint64_t* full_bar = bars;
   uint64_t* empty_bar = bars + NUM_STAGES;
-  uint64_t* res_full = bars + 2 * NUM_STAGES;
-  uint8_t* staging = smem + L::OFF_STAGING;
-  float* stats_sm = reinterpret_cast<float*>(smem + L::OFF_STATS);
 
-  const int warp = threadIdx.x >> 5;
+  const int warp = __shfl_sync(0xffffffffu, threadIdx.x >> 5, 0);   // provably warp-uniform: ptxas sizes each setmaxnreg region
   const int lane = threadIdx.x & 31;
   pdl_trigger();
 
-  // full: the TMA transaction arrival (+ the 128 producer threads' arrivals when FUSED); empty: one arrival per consumer warp
+  // full: the TMA transaction arrival (+ the 128 producer threads' arrivals when FUSED); empty: one arrival per warp
+  // of the consumer warpgroup that read the stage
   constexpr uint32_t FULL_COUNT = FUSED ? 1 + 128 : 1;
   if (threadIdx.x == 0) {
     tma_prefetch_desc(&map_a0);
@@ -184,8 +195,9 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap map_a0, const __grid_constant
     if (P.nseg > 1) tma_prefetch_desc(&map_a1);
     if (P.nseg > 2) tma_prefetch_desc(&map_a2);
     if (P.has_residual) tma_prefetch_desc(&map_r);
-    for (int i = 0; i < NUM_STAGES; ++i) { mbar_init(&full_bar[i], FULL_COUNT); mbar_init(&empty_bar[i], NUM_CONS / 32); }
-    mbar_init(res_full, 1);
+    for (int i = 0; i < NUM_STAGES; ++i) { mbar_init(&full_bar[i], FULL_COUNT); mbar_init(&empty_bar[i], 4); }
+    mbar_init(bars + 2 * NUM_STAGES, 1);
+    mbar_init(bars + 2 * NUM_STAGES + 1, 1);
     mbar_fence_init();
   }
   __syncthreads();
@@ -193,10 +205,12 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap map_a0, const __grid_constant
 
   if (warp < 4) {
     // =========================== producer (warpgroup 0) ===========================
+    setmaxnreg_dec<R::PRODUCER>();
     const int pt = threadIdx.x;                 // 0..127
     if (!FUSED && pt != 0) return;
-    int stage = 0; uint32_t phase = 0;
-    for (int tile = blockIdx.x; tile < P.num_tiles; tile += gridDim.x) {
+    const int n_local = tc_local_tiles(blockIdx.x, gridDim.x, P.num_tiles);
+    for (int j = 0; j < n_local; ++j) {
+      const int tile = blockIdx.x + j * gridDim.x;
       const int m_tile = tile % P.num_m_tiles, n_tile = tile / P.num_m_tiles;
       const int tx = m_tile % P.tiles_w, ty = (m_tile / P.tiles_w) % P.tiles_h, tn = m_tile / (P.tiles_w * P.tiles_h);
       const int x0 = tx * P.bw, y0 = ty * P.bh, n0 = tn * P.bn;
@@ -207,22 +221,22 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap map_a0, const __grid_constant
         for (int tap = 0; tap < taps; ++tap) {
           const int dy = taps == 9 ? tap / 3 - 1 : 0, dx = taps == 9 ? tap % 3 - 1 : 0;
           for (int ch = 0; ch < P.seg_chunks[s]; ++ch, ++kb) {
-            mbar_wait(&empty_bar[stage], phase ^ 1, P.dbg, 100 + stage);
-            uint8_t* sa = smem + stage * L::STAGE_BYTES;
+            const TcSlot sl = tc_slot(j, kb, P.num_k_blocks, NUM_STAGES);
+            mbar_wait(&empty_bar[sl.stage], sl.phase ^ 1, P.dbg, 100 + sl.stage);
+            uint8_t* sa = smem + sl.stage * L::STAGE_BYTES;
             const bool build_a = FUSED && s == 0;
             if (pt == 0) {
-              mbar_arrive_expect_tx(&full_bar[stage], build_a ? L::B_TILE_BYTES : L::STAGE_BYTES);
-              if (!build_a) tma_load_4d(sa, ma, &full_bar[stage], ch * BLOCK_K, x0 + dx, y0 + dy, n0);
-              tma_load_2d(sa + A_TILE_BYTES, &map_b, &full_bar[stage], kb * BLOCK_K, n_tile * BLOCK_N);
+              mbar_arrive_expect_tx(&full_bar[sl.stage], build_a ? L::B_TILE_BYTES : L::STAGE_BYTES);
+              if (!build_a) tma_load_4d(sa, ma, &full_bar[sl.stage], ch * BLOCK_K, x0 + dx, y0 + dy, n0);
+              tma_load_2d(sa + A_TILE_BYTES, &map_b, &full_bar[sl.stage], kb * BLOCK_K, n_tile * BLOCK_N);
             }
             if (FUSED) {
               if (build_a) {
                 fused_a_row(sa, pt, P, x0, y0, n0, dx, dy, ch);
                 fence_proxy_async_smem();          // generic-proxy smem writes -> visible to wgmma (async proxy)
               }
-              mbar_arrive(&full_bar[stage]);
+              mbar_arrive(&full_bar[sl.stage]);
             }
-            if (++stage == NUM_STAGES) { stage = 0; phase ^= 1; }
           }
         }
       }
@@ -231,22 +245,31 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap map_a0, const __grid_constant
   }
 
   // =========================== MMA + epilogue (warpgroups 1, 2) ===========================
-  const int ct = threadIdx.x - 128;            // 0..255
-  const int wg = ct >> 7;                      // rows [64 wg, 64 wg + 64) of the tile
-  const int wt = ct & 127;
+  setmaxnreg_inc<R::CONSUMER>();
+  const int wg = warp / 4 - 1;                 // consumer warpgroup: takes the local tiles j with tc_consumer_of(j) == wg
+  const int wt = threadIdx.x & 127;
   const int rps = P.bw * P.bh;                 // rows per sample inside a tile
-  int stage = 0; uint32_t phase = 0; uint32_t res_phase = 0;
-  float acc[BLOCK_N / 2];
-  for (int tile = blockIdx.x; tile < P.num_tiles; tile += gridDim.x) {
+  uint8_t* staging = smem + L::OFF_STAGING + wg * L::STAGING_BYTES;
+  float* stats_sm = reinterpret_cast<float*>(smem + L::OFF_STATS + wg * L::STATS_BYTES);
+  uint64_t* res_full = bars + 2 * NUM_STAGES + wg;
+  // named barriers: 1 + wg = this warpgroup's epilogue (128 threads); 3 + wg = "warpgroup wg may issue its MMAs", which
+  // the other warpgroup arrives on once its own mainloop has issued (256 threads: 128 arrive, 128 sync)
+  const int epi_bar = 1 + wg, my_turn = 3 + wg, other_turn = 4 - wg;
+  const int n_local = tc_local_tiles(blockIdx.x, gridDim.x, P.num_tiles);
+  uint32_t res_phase = 0;
+  float acc[2][BLOCK_N / 2];                   // rows 0-63, rows 64-127 of the tile
+  for (int j = 0; j < n_local; ++j) {
+    if (tc_consumer_of(j) != wg) continue;
+    const int tile = blockIdx.x + j * gridDim.x;
     const int m_tile = tile % P.num_m_tiles, n_tile = tile / P.num_m_tiles;
     const int tx = m_tile % P.tiles_w, ty = (m_tile / P.tiles_w) % P.tiles_h, tn = m_tile / (P.tiles_w * P.tiles_h);
     const int x0 = tx * P.bw, y0 = ty * P.bh, n0 = tn * P.bn;
     const int c_tile = n_tile * BLOCK_N;
 
-    // staging buffer must be free: the previous tile's TMA store has finished reading it, every thread is done with it
-    if (ct == 0) tma_store_wait_read0();
-    named_bar_sync(1, NUM_CONS);
-    if (P.has_residual && ct == 0) {           // the residual tile lands in the staging buffer while the MMAs run
+    // staging buffer must be free: this warpgroup's previous TMA store has finished reading it, every thread is done with it
+    if (wt == 0) tma_store_wait_read0();
+    named_bar_sync(epi_bar, 128);
+    if (P.has_residual && wt == 0) {           // the residual tile lands in the staging buffer while the MMAs run
       fence_proxy_async_smem();
       mbar_arrive_expect_tx(res_full, L::STAGING_BYTES);
 #pragma unroll
@@ -254,59 +277,68 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap map_a0, const __grid_constant
         tma_load_4d(staging + c * A_TILE_BYTES, &map_r, res_full, c_tile + c * 64, x0, y0, n0);
     }
 
+    // the other warpgroup has waited for every stage of the tile before this one: the ring's parities are unambiguous
+    if (j > 0) named_bar_sync(my_turn, 256);
     int prev = -1;
     for (int kb = 0; kb < P.num_k_blocks; ++kb) {
-      mbar_wait(&full_bar[stage], phase, P.dbg, 300 + stage);
-      const uint32_t a_addr = smem_u32(smem + stage * L::STAGE_BYTES);
-      const uint64_t adesc = make_smem_desc(a_addr + wg * 64 * 128);
+      const TcSlot sl = tc_slot(j, kb, P.num_k_blocks, NUM_STAGES);
+      mbar_wait(&full_bar[sl.stage], sl.phase, P.dbg, 300 + 10 * wg + sl.stage);
+      const uint32_t a_addr = smem_u32(smem + sl.stage * L::STAGE_BYTES);
+      const uint64_t adesc = make_smem_desc(a_addr);
       const uint64_t bdesc = make_smem_desc(a_addr + A_TILE_BYTES);
       wgmma_fence();
 #pragma unroll
-      for (int k = 0; k < BLOCK_K / WG_K; ++k)
-        // advance 16 fp16 = 32 B along K inside the 128 B swizzle row: +2 in the (addr >> 4) field
-        wgmma_tile<BLOCK_N>(acc, adesc + (uint64_t)(2 * k), bdesc + (uint64_t)(2 * k), (kb | k) != 0);
+      for (int k = 0; k < BLOCK_K / WG_K; ++k) {
+        // advance 16 fp16 = 32 B along K inside the 128 B swizzle row: +2 in the (addr >> 4) field; rows 64-127 start
+        // 64 x 128 B = 8 KB (+512) further
+        wgmma_tile<BLOCK_N>(acc[0], adesc + (uint64_t)(2 * k), bdesc + (uint64_t)(2 * k), (kb | k) != 0);
+        wgmma_tile<BLOCK_N>(acc[1], adesc + (uint64_t)(512 + 2 * k), bdesc + (uint64_t)(2 * k), (kb | k) != 0);
+      }
       wgmma_commit();
       wgmma_wait<1>();                         // the previous k-block's MMAs have retired: its stage is free
       if (prev >= 0) { __syncwarp(); if (lane == 0) mbar_arrive(&empty_bar[prev]); }
-      prev = stage;
-      if (++stage == NUM_STAGES) { stage = 0; phase ^= 1; }
+      prev = sl.stage;
     }
+    if (j + 1 < n_local) named_bar_arrive(other_turn, 256);
     wgmma_wait<0>();
     __syncwarp();
     if (lane == 0) mbar_arrive(&empty_bar[prev]);
 
     if (P.has_residual) {
-      mbar_wait(res_full, res_phase, P.dbg, 400);
+      mbar_wait(res_full, res_phase, P.dbg, 400 + wg);
       res_phase ^= 1;
     }
     // accumulator fragment of m64nN: thread wt holds rows 16 (wt / 32) + (lane / 4) + {0, 8}, columns 8 j + 2 (lane % 4) + {0, 1}
     const float* bias_row = P.bias ? P.bias + c_tile : nullptr;
 #pragma unroll
-    for (int h = 0; h < 2; ++h) {
-      const int row = wg * 64 + (wt >> 5) * 16 + (lane >> 2) + 8 * h;
-      int n_s = n0 + row / rps;
-      if (n_s >= P.N) n_s = P.N - 1;            // rows of a partially out-of-range box (never stored)
-      const float* temb_row = P.temb ? P.temb + (size_t)n_s * P.temb_stride + c_tile : nullptr;
-      uint8_t* my_row = staging + row * 128 + (lane & 3) * 4;
-      const int sw = row & 7;
+    for (int m = 0; m < 2; ++m) {
 #pragma unroll
-      for (int j = 0; j < BLOCK_N / 8; ++j) {
-        const int cb = j * 8 + (lane & 3) * 2;   // channel inside the tile
-        float v0 = acc[4 * j + 2 * h], v1 = acc[4 * j + 2 * h + 1];
-        if (bias_row) { v0 += __ldg(bias_row + cb); v1 += __ldg(bias_row + cb + 1); }
-        if (temb_row) { v0 += __ldg(temb_row + cb); v1 += __ldg(temb_row + cb + 1); }
-        __half2* sp = reinterpret_cast<__half2*>(my_row + (j >> 3) * A_TILE_BYTES + (((j & 7) ^ sw) << 4));
-        if (P.has_residual) {
-          const float2 f = __half22float2(*sp);
-          v0 += f.x; v1 += f.y;
+      for (int h = 0; h < 2; ++h) {
+        const int row = m * 64 + (wt >> 5) * 16 + (lane >> 2) + 8 * h;
+        int n_s = n0 + row / rps;
+        if (n_s >= P.N) n_s = P.N - 1;            // rows of a partially out-of-range box (never stored)
+        const float* temb_row = P.temb ? P.temb + (size_t)n_s * P.temb_stride + c_tile : nullptr;
+        uint8_t* my_row = staging + row * 128 + (lane & 3) * 4;
+        const int sw = row & 7;
+#pragma unroll
+        for (int jj = 0; jj < BLOCK_N / 8; ++jj) {
+          const int cb = jj * 8 + (lane & 3) * 2;  // channel inside the tile
+          float v0 = acc[m][4 * jj + 2 * h], v1 = acc[m][4 * jj + 2 * h + 1];
+          if (bias_row) { v0 += __ldg(bias_row + cb); v1 += __ldg(bias_row + cb + 1); }
+          if (temb_row) { v0 += __ldg(temb_row + cb); v1 += __ldg(temb_row + cb + 1); }
+          __half2* sp = reinterpret_cast<__half2*>(my_row + (jj >> 3) * A_TILE_BYTES + (((jj & 7) ^ sw) << 4));
+          if (P.has_residual) {
+            const float2 f = __half22float2(*sp);
+            v0 += f.x; v1 += f.y;
+          }
+          *sp = __floats2half2_rn(v0 * P.scale, v1 * P.scale);
         }
-        *sp = __floats2half2_rn(v0 * P.scale, v1 * P.scale);
       }
     }
 
     fence_proxy_async_smem();
-    named_bar_sync(1, NUM_CONS);
-    if (ct == 0) {
+    named_bar_sync(epi_bar, 128);
+    if (wt == 0) {
 #pragma unroll
       for (int c = 0; c < L::N_CHUNKS; ++c)
         tma_store_4d(&map_d, staging + c * A_TILE_BYTES, c_tile + c * 64, x0, y0, n0);
@@ -314,36 +346,34 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap map_a0, const __grid_constant
     }
 
     if (P.stats) {
-      // per-channel (sum, sum^2) over each 32-row segment, from the fp16 values actually stored
-      if (ct < 128) {
-        const int seg = ct >> 5;
+      // per-channel (sum, sum^2) over each 32-row segment (one per warp), from the fp16 values actually stored
+      const int seg = wt >> 5;
 #pragma unroll
-        for (int c = 0; c < L::N_CHUNKS; ++c) {
-          float s0 = 0.f, q0 = 0.f, s1 = 0.f, q1 = 0.f;
-          const uint8_t* cbase = staging + c * A_TILE_BYTES;
+      for (int c = 0; c < L::N_CHUNKS; ++c) {
+        float s0 = 0.f, q0 = 0.f, s1 = 0.f, q1 = 0.f;
+        const uint8_t* cbase = staging + c * A_TILE_BYTES;
 #pragma unroll 8
-          for (int rr = 0; rr < 32; ++rr) {
-            const int r2 = seg * 32 + rr;
-            const __half2 hv = *reinterpret_cast<const __half2*>(cbase + r2 * 128 + ((((lane >> 2) ^ (r2 & 7)) << 4) | ((lane & 3) << 2)));
-            const float2 f = __half22float2(hv);
-            s0 += f.x; q0 += f.x * f.x; s1 += f.y; q1 += f.y * f.y;
-          }
-          float* d = stats_sm + ((seg * BLOCK_N) + c * 64 + lane * 2) * 2;
-          d[0] = s0; d[1] = q0; d[2] = s1; d[3] = q1;
+        for (int rr = 0; rr < 32; ++rr) {
+          const int r2 = seg * 32 + rr;
+          const __half2 hv = *reinterpret_cast<const __half2*>(cbase + r2 * 128 + ((((lane >> 2) ^ (r2 & 7)) << 4) | ((lane & 3) << 2)));
+          const float2 f = __half22float2(hv);
+          s0 += f.x; q0 += f.x * f.x; s1 += f.y; q1 += f.y * f.y;
         }
+        float* d = stats_sm + ((seg * BLOCK_N) + c * 64 + lane * 2) * 2;
+        d[0] = s0; d[1] = q0; d[2] = s1; d[3] = q1;
       }
-      named_bar_sync(1, NUM_CONS);
+      named_bar_sync(epi_bar, 128);
       const int groups = rps >= 128 ? 1 : 128 / rps;       // samples covered by this tile
       const int spg = 4 / groups;                          // 32-row segments per sample
       const int slot = ty * P.tiles_w + tx;
-      for (int c = ct; c < BLOCK_N; c += NUM_CONS) {
+      for (int c = wt; c < BLOCK_N; c += 128) {
         for (int g = 0; g < groups; ++g) {
           const int n = n0 + g;
           if (n >= P.N) break;
           float s = 0.f, q = 0.f;
-          for (int j = 0; j < spg; ++j) {
-            s += stats_sm[(((g * spg + j) * BLOCK_N) + c) * 2];
-            q += stats_sm[(((g * spg + j) * BLOCK_N) + c) * 2 + 1];
+          for (int jj = 0; jj < spg; ++jj) {
+            s += stats_sm[(((g * spg + jj) * BLOCK_N) + c) * 2];
+            q += stats_sm[(((g * spg + jj) * BLOCK_N) + c) * 2 + 1];
           }
           float* d = P.stats + (((size_t)n * P.slots + slot) * P.Cout + c_tile + c) * 2;
           d[0] = s; d[1] = q;
@@ -351,7 +381,7 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap map_a0, const __grid_constant
       }
     }
   }
-  if (ct == 0) tma_store_wait_all0();
+  if (wt == 0) tma_store_wait_all0();
 }
 
 }  // namespace
@@ -489,10 +519,10 @@ void launch_width(cudaStream_t st, const ConvArgs& a, TensorDesc& out, int* dbg)
     int bw, bh, bn;
     choose_box(out.H, out.W, bw, bh, bn);
     const int tiles128 = (out.W / bw) * (out.H / bh) * cdiv(out.N, bn) * (out.C / 128);
-    if (tiles128 * 2 <= num_sms()) { launch_impl<64, 6, FUSED>(st, a, out, dbg); return; }
+    if (tiles128 * 2 <= num_sms()) { launch_impl<64, 7, FUSED>(st, a, out, dbg); return; }
   }
-  if (out.C % 128 == 0) launch_impl<128, 5, FUSED>(st, a, out, dbg);
-  else launch_impl<64, 6, FUSED>(st, a, out, dbg);
+  if (out.C % 128 == 0) launch_impl<128, 4, FUSED>(st, a, out, dbg);
+  else launch_impl<64, 7, FUSED>(st, a, out, dbg);
 }
 
 }  // namespace
