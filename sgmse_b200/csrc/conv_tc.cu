@@ -44,6 +44,7 @@ constexpr int BLOCK_K = 64;     // fp16 elements = 128 B = one swizzle row
 constexpr int WG_K = 16;
 constexpr int NUM_THREADS = 384;
 constexpr int A_TILE_BYTES = BLOCK_M * BLOCK_K * 2;   // 16 KB
+constexpr int STAGES_N128 = 4, STAGES_N64 = 7;        // ring depth of the 128- and 64-wide channel tiles
 
 struct TcParams {
   int tiles_w, tiles_h, tiles_n;
@@ -459,13 +460,27 @@ int num_sms() {
   return n;
 }
 
+TcPlan conv_tc_plan(const TensorDesc& out, int sms, bool narrow) {
+  TcPlan p;
+  if (!choose_box(out.H, out.W, p.bw, p.bh, p.bn)) return TcPlan{};
+  const int m_tiles = (out.W / p.bw) * (out.H / p.bh) * cdiv(out.N, p.bn);
+  // tc1_narrow: when 128-wide channel tiles would fill less than half the SMs, 64-wide tiles double the CTAs.  The
+  // accumulation order of an output element does not depend on the tile width: bit-identical.
+  const bool wide = out.C % 128 == 0 && !(narrow && m_tiles * (out.C / 128) * 2 <= sms);
+  p.block_n = wide ? 128 : 64;
+  p.stages = wide ? STAGES_N128 : STAGES_N64;
+  p.tiles = m_tiles * (out.C / p.block_n);
+  p.grid = p.tiles < sms ? p.tiles : sms;
+  if (p.grid > 0) { p.min_local = p.tiles / p.grid; p.max_local = cdiv(p.tiles, p.grid); }
+  return p;
+}
+
 namespace {
 
 template <int BLOCK_N, int NUM_STAGES, bool FUSED>
-void launch_impl(cudaStream_t st, const ConvArgs& a, TensorDesc& out, int* dbg) {
+void launch_impl(cudaStream_t st, const ConvArgs& a, TensorDesc& out, int* dbg, const TcPlan& plan) {
   using L = SmemLayout<BLOCK_N, NUM_STAGES>;
-  int bw, bh, bn;
-  SG_CHECK(choose_box(out.H, out.W, bw, bh, bn), "conv_tc: no 128-pixel box for %dx%d", out.H, out.W);
+  const int bw = plan.bw, bh = plan.bh, bn = plan.bn;
   TcParams P{};
   P.bw = bw; P.bh = bh; P.bn = bn;
   P.tiles_w = out.W / bw; P.tiles_h = out.H / bh; P.tiles_n = cdiv(out.N, bn);
@@ -506,23 +521,16 @@ void launch_impl(cudaStream_t st, const ConvArgs& a, TensorDesc& out, int* dbg) 
   if (first_use_on_device(attr_devs)) {
     CUDA_OK(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, L::DYN_BYTES));
   }
-  const int grid = P.num_tiles < num_sms() ? P.num_tiles : num_sms();
-  launch_k(kern, dim3(grid), dim3(NUM_THREADS), (size_t)L::DYN_BYTES, st, ma[0], ma[1], ma[2], mb, md, mr, P);
+  launch_k(kern, dim3(plan.grid), dim3(NUM_THREADS), (size_t)L::DYN_BYTES, st, ma[0], ma[1], ma[2], mb, md, mr, P);
   CUDA_OK(cudaGetLastError());
 }
 
 template <bool FUSED>
 void launch_width(cudaStream_t st, const ConvArgs& a, TensorDesc& out, int* dbg) {
-  // tc1_narrow: when 128-wide channel tiles would fill less than half the SMs, 64-wide tiles double the CTAs.  The
-  // accumulation order of an output element does not depend on the tile width: bit-identical.
-  if (out.C % 128 == 0 && g_tc1_narrow) {
-    int bw, bh, bn;
-    choose_box(out.H, out.W, bw, bh, bn);
-    const int tiles128 = (out.W / bw) * (out.H / bh) * cdiv(out.N, bn) * (out.C / 128);
-    if (tiles128 * 2 <= num_sms()) { launch_impl<64, 7, FUSED>(st, a, out, dbg); return; }
-  }
-  if (out.C % 128 == 0) launch_impl<128, 4, FUSED>(st, a, out, dbg);
-  else launch_impl<64, 7, FUSED>(st, a, out, dbg);
+  const TcPlan plan = conv_tc_plan(out, num_sms(), g_tc1_narrow != 0);
+  SG_CHECK(plan.bw > 0, "conv_tc: no 128-pixel box for %dx%d", out.H, out.W);
+  if (plan.block_n == 128) launch_impl<128, STAGES_N128, FUSED>(st, a, out, dbg, plan);
+  else launch_impl<64, STAGES_N64, FUSED>(st, a, out, dbg, plan);
 }
 
 }  // namespace

@@ -76,6 +76,15 @@ bool conv_tc_supported(const ConvArgs& a, const TensorDesc& out);
 // shape test of the fused GroupNorm-apply/SiLU form (3x3 over c0 [+ c1] raw channels), usable before the tensors exist
 bool conv_tc_fuse_shape_ok(int H, int W, int c0, int c1, int cout);
 void launch_conv_tc(cudaStream_t st, const ConvArgs& a, TensorDesc& out, int* dbg_flag);
+// Launch plan of conv_tc for an output tensor: the host-side decision launch_conv_tc acts on.
+struct TcPlan {
+  int bw = 0, bh = 0, bn = 0;          // pixel box of one 128-row tile (bw * bh * bn = 128); bw == 0: no box fits H x W
+  int block_n = 0, stages = 0;         // channel tile width, shared-memory ring depth
+  int tiles = 0, grid = 0;             // output tiles, persistent CTAs
+  int min_local = 0, max_local = 0;    // tiles per CTA
+};
+// sms: multiprocessors the grid is sized for; narrow: g_tc1_narrow
+TcPlan conv_tc_plan(const TensorDesc& out, int sms, bool narrow);
 extern thread_local int g_tc1_narrow;   // 1: 64-wide channel tiles when 128-wide ones fill less than half the SMs (the default)
 extern thread_local int g_tc_variant;   // 0: TMA-fed convolutions, separate gn_apply launches; 5: GroupNorm+SiLU fused into the 3x3
                                         // convolutions where the shape allows (its producer re-evaluates every tap: 3.2x slower per benchmark step on H100)
