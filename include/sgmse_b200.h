@@ -54,8 +54,11 @@ typedef struct sgmse_b200_engine sgmse_b200_engine;
 enum { SGMSE_B200_BACKBONE_NCSNPP = 0, SGMSE_B200_BACKBONE_NCSNPP_48K = 1, SGMSE_B200_BACKBONE_NCSNPP_V2 = 2 };
 /* arithmetic mode: 0 = fp32 activations, CUDA-core convolutions (validation);
  *                  1 = fp16 activations, CUDA-core convolutions (debug);
- *                  2 = fp16 activations, wgmma tensor-core convolutions (product path) */
-enum { SGMSE_B200_MODE_FP32 = 0, SGMSE_B200_MODE_FP16_DIRECT = 1, SGMSE_B200_MODE_FP16_TC = 2 };
+ *                  2 = fp16 activations, wgmma tensor-core convolutions (product path);
+ *                  3 = fp32 activations, wgmma tensor-core convolutions with TF32 operands (10-bit mantissas, fp32
+ *                      accumulation and fp32 residual stream): the fp32 range of mode 0 at tensor-core rates, and no fp16
+ *                      range events.  Its workspace is that of mode 0, about twice that of mode 2. */
+enum { SGMSE_B200_MODE_FP32 = 0, SGMSE_B200_MODE_FP16_DIRECT = 1, SGMSE_B200_MODE_FP16_TC = 2, SGMSE_B200_MODE_TF32_TC = 3 };
 enum { SGMSE_B200_PRED_REVERSE_DIFFUSION = 0, SGMSE_B200_PRED_EULER_MARUYAMA = 1, SGMSE_B200_PRED_NONE = 2 };
 enum { SGMSE_B200_CORR_ALD = 0, SGMSE_B200_CORR_LANGEVIN = 1, SGMSE_B200_CORR_NONE = 2 };
 enum { SGMSE_B200_PAD_ZERO = 0, SGMSE_B200_PAD_REFLECTION = 1 };

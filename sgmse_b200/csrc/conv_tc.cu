@@ -1,4 +1,5 @@
-// wgmma implicit-GEMM convolution for sm_90a (3x3 pad-1 / 1x1, NHWC fp16 -> fp16, fp32 accumulate in registers).
+// wgmma implicit-GEMM convolution for sm_90a (3x3 pad-1 / 1x1, NHWC fp16 -> fp16, fp32 accumulate in registers; or
+// NHWC fp32 -> fp32 with TF32 operands, see "TF32" below).
 //
 //   D[pixel, cout] = sum_{segment, tap, cin} A_seg[pixel + tap offset, cin] * W[cout, (segment, tap, cin)]
 //
@@ -27,6 +28,13 @@
 // (seg[0].src, concatenated with gn_cat), so the gn_apply pass and its buffer disappear.  Out-of-image taps read 0
 // (the padding of the ACTIVATED tensor, as in F.conv2d after the activation).
 //
+// TF32 (T = float, mode tf32_tc): the same ring, descriptors and schedule in bytes.  One 128 B swizzle row holds 32 fp32
+// channels, so a K block is 32 channels of one tap and a wgmma m64n64k8 TF32 step covers 8 (4 steps per block, +32 B each,
+// as for fp16).  The tensor cores read the upper 19 bits of each fp32 operand; the weights are stored RNA-rounded to TF32
+// (tf32_rna), the activations go in as stored.  The epilogue stages fp32 (32 channels per 128 B row), adds bias, time
+// embedding and the fp32 residual, and reduces the GroupNorm partials from the staged fp32 values.  Tiles are 64 channels
+// wide (fp32 staging is twice the bytes) and the fused GroupNorm producer is fp16 only.
+//
 // Reference semantics: F.conv2d calls of ResnetBlockBigGANpp.forward (layerspp.py:260-269) and NIN
 // (layers.py:546-555); the epilogue fuses `h += Dense_0(act(temb))[:, :, None, None]`, the Conv_2
 // shortcut add and `(x + h) / sqrt(2)` (layerspp.py:262-274).
@@ -40,11 +48,15 @@ namespace sgmse {
 namespace {
 
 constexpr int BLOCK_M = 128;
-constexpr int BLOCK_K = 64;     // fp16 elements = 128 B = one swizzle row
-constexpr int WG_K = 16;
+constexpr int ROW_BYTES = 128;  // one SWIZZLE_128B row: the K extent of one k-block
+// channels of one k-block (one swizzle row) and of one wgmma K step (32 B): 64 / 16 fp16, 32 / 8 fp32 (TF32)
+template <typename T> constexpr int kBlockK = ROW_BYTES / (int)sizeof(T);
+template <typename T> constexpr int kWgK = 32 / (int)sizeof(T);
+constexpr int BLOCK_K = kBlockK<__half>;              // the fused producer (fp16 only)
 constexpr int NUM_THREADS = 384;
-constexpr int A_TILE_BYTES = BLOCK_M * BLOCK_K * 2;   // 16 KB
-constexpr int STAGES_N128 = 4, STAGES_N64 = 7;        // ring depth of the 128- and 64-wide channel tiles
+constexpr int A_TILE_BYTES = BLOCK_M * ROW_BYTES;     // 16 KB
+constexpr int STAGES_N128 = 4, STAGES_N64 = 7;        // ring depth of the 128- and 64-wide channel tiles (fp16)
+constexpr int STAGES_TF32 = 6;                        // ring depth of the 64-wide fp32 tiles (two 32 KB staging buffers)
 
 struct TcParams {
   int tiles_w, tiles_h, tiles_n;
@@ -70,11 +82,11 @@ struct TcParams {
   int* dbg;
 };
 
-template <int BLOCK_N, int NUM_STAGES>
+template <int BLOCK_N, int NUM_STAGES, int ESIZE = 2>   // ESIZE: bytes per activation element (2 fp16, 4 fp32)
 struct SmemLayout {
-  static constexpr int B_TILE_BYTES = BLOCK_N * BLOCK_K * 2;
+  static constexpr int B_TILE_BYTES = BLOCK_N * ROW_BYTES;
   static constexpr int STAGE_BYTES = A_TILE_BYTES + B_TILE_BYTES;
-  static constexpr int N_CHUNKS = BLOCK_N / 64;
+  static constexpr int N_CHUNKS = BLOCK_N * ESIZE / ROW_BYTES;          // 128 B-row output chunks of the staged tile
   static constexpr int STAGING_BYTES = N_CHUNKS * A_TILE_BYTES;         // per consumer warpgroup
   static constexpr int STATS_BYTES = 4 * BLOCK_N * 2 * 4;               // per consumer warpgroup: float [4][BLOCK_N][2]
   static constexpr int OFF_STAGING = NUM_STAGES * STAGE_BYTES;
@@ -120,9 +132,20 @@ __device__ __forceinline__ void wgmma_m64n64k16(float (&d)[32], uint64_t da, uin
       : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31])
       : "l"(da), "l"(db), "r"(accumulate));
 }
-template <int BLOCK_N>
+// the same with TF32 operands (K = 8): no transpose immediates; both operands are K-major
+__device__ __forceinline__ void wgmma_m64n64k8_tf32(float (&d)[32], uint64_t da, uint64_t db, uint32_t accumulate) {
+  asm volatile(
+      "{\n\t.reg .pred p;\n\t"
+      "setp.ne.b32 p, %34, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n64k8.f32.tf32.tf32 "
+      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, %32, %33, p, 1, 1;\n\t}"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31])
+      : "l"(da), "l"(db), "r"(accumulate));
+}
+template <int BLOCK_N, typename T>
 __device__ __forceinline__ void wgmma_tile(float (&d)[BLOCK_N / 2], uint64_t da, uint64_t db, uint32_t accumulate) {
-  if constexpr (BLOCK_N == 128) wgmma_m64n128k16(d, da, db, accumulate);
+  if constexpr (sizeof(T) == 4) wgmma_m64n64k8_tf32(d, da, db, accumulate);
+  else if constexpr (BLOCK_N == 128) wgmma_m64n128k16(d, da, db, accumulate);
   else wgmma_m64n64k16(d, da, db, accumulate);
 }
 
@@ -166,14 +189,17 @@ template <bool FUSED> struct TcRegs;
 template <> struct TcRegs<false> { static constexpr int PRODUCER = 40, CONSUMER = 232; };
 template <> struct TcRegs<true> { static constexpr int PRODUCER = 56, CONSUMER = 224; };
 
-template <int BLOCK_N, int NUM_STAGES, bool FUSED>
+template <int BLOCK_N, int NUM_STAGES, bool FUSED, typename T>
 __global__ void __launch_bounds__(NUM_THREADS, 1)
 conv_tc_kernel(const __grid_constant__ CUtensorMap map_a0, const __grid_constant__ CUtensorMap map_a1,
                const __grid_constant__ CUtensorMap map_a2, const __grid_constant__ CUtensorMap map_b,
                const __grid_constant__ CUtensorMap map_d, const __grid_constant__ CUtensorMap map_r,
                const TcParams P) {
-  using L = SmemLayout<BLOCK_N, NUM_STAGES>;
+  using L = SmemLayout<BLOCK_N, NUM_STAGES, sizeof(T)>;
   using R = TcRegs<FUSED>;
+  constexpr bool TF32 = sizeof(T) == 4;
+  constexpr int BK = kBlockK<T>, WK = kWgK<T>;
+  static_assert(!TF32 || (BLOCK_N == 64 && !FUSED), "conv_tc: TF32 tiles are 64 wide, with TMA-fed operands");
   static_assert(128 * R::PRODUCER + 256 * R::CONSUMER <= NUM_THREADS * 168, "conv_tc: register budgets over the CTA's");
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023);
@@ -228,8 +254,8 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap map_a0, const __grid_constant
             const bool build_a = FUSED && s == 0;
             if (pt == 0) {
               mbar_arrive_expect_tx(&full_bar[sl.stage], build_a ? L::B_TILE_BYTES : L::STAGE_BYTES);
-              if (!build_a) tma_load_4d(sa, ma, &full_bar[sl.stage], ch * BLOCK_K, x0 + dx, y0 + dy, n0);
-              tma_load_2d(sa + A_TILE_BYTES, &map_b, &full_bar[sl.stage], kb * BLOCK_K, n_tile * BLOCK_N);
+              if (!build_a) tma_load_4d(sa, ma, &full_bar[sl.stage], ch * BK, x0 + dx, y0 + dy, n0);
+              tma_load_2d(sa + A_TILE_BYTES, &map_b, &full_bar[sl.stage], kb * BK, n_tile * BLOCK_N);
             }
             if (FUSED) {
               if (build_a) {
@@ -275,7 +301,7 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap map_a0, const __grid_constant
       mbar_arrive_expect_tx(res_full, L::STAGING_BYTES);
 #pragma unroll
       for (int c = 0; c < L::N_CHUNKS; ++c)
-        tma_load_4d(staging + c * A_TILE_BYTES, &map_r, res_full, c_tile + c * 64, x0, y0, n0);
+        tma_load_4d(staging + c * A_TILE_BYTES, &map_r, res_full, c_tile + c * BK, x0, y0, n0);
     }
 
     // the other warpgroup has waited for every stage of the tile before this one: the ring's parities are unambiguous
@@ -289,11 +315,11 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap map_a0, const __grid_constant
       const uint64_t bdesc = make_smem_desc(a_addr + A_TILE_BYTES);
       wgmma_fence();
 #pragma unroll
-      for (int k = 0; k < BLOCK_K / WG_K; ++k) {
-        // advance 16 fp16 = 32 B along K inside the 128 B swizzle row: +2 in the (addr >> 4) field; rows 64-127 start
-        // 64 x 128 B = 8 KB (+512) further
-        wgmma_tile<BLOCK_N>(acc[0], adesc + (uint64_t)(2 * k), bdesc + (uint64_t)(2 * k), (kb | k) != 0);
-        wgmma_tile<BLOCK_N>(acc[1], adesc + (uint64_t)(512 + 2 * k), bdesc + (uint64_t)(2 * k), (kb | k) != 0);
+      for (int k = 0; k < BK / WK; ++k) {
+        // advance 16 fp16 (8 fp32) = 32 B along K inside the 128 B swizzle row: +2 in the (addr >> 4) field; rows 64-127
+        // start 64 x 128 B = 8 KB (+512) further
+        wgmma_tile<BLOCK_N, T>(acc[0], adesc + (uint64_t)(2 * k), bdesc + (uint64_t)(2 * k), (kb | k) != 0);
+        wgmma_tile<BLOCK_N, T>(acc[1], adesc + (uint64_t)(512 + 2 * k), bdesc + (uint64_t)(2 * k), (kb | k) != 0);
       }
       wgmma_commit();
       wgmma_wait<1>();                         // the previous k-block's MMAs have retired: its stage is free
@@ -319,20 +345,40 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap map_a0, const __grid_constant
         int n_s = n0 + row / rps;
         if (n_s >= P.N) n_s = P.N - 1;            // rows of a partially out-of-range box (never stored)
         const float* temb_row = P.temb ? P.temb + (size_t)n_s * P.temb_stride + c_tile : nullptr;
-        uint8_t* my_row = staging + row * 128 + (lane & 3) * 4;
-        const int sw = row & 7;
+        if constexpr (TF32) {
+          // fp32 staging: 32 channels per 128 B row; channels cb, cb + 1 are 8 bytes of 16-byte unit (cb % 32) / 4
+          uint8_t* my_row = staging + row * 128 + (lane & 1) * 8;
+          const int sw = row & 7;
 #pragma unroll
-        for (int jj = 0; jj < BLOCK_N / 8; ++jj) {
-          const int cb = jj * 8 + (lane & 3) * 2;  // channel inside the tile
-          float v0 = acc[m][4 * jj + 2 * h], v1 = acc[m][4 * jj + 2 * h + 1];
-          if (bias_row) { v0 += __ldg(bias_row + cb); v1 += __ldg(bias_row + cb + 1); }
-          if (temb_row) { v0 += __ldg(temb_row + cb); v1 += __ldg(temb_row + cb + 1); }
-          __half2* sp = reinterpret_cast<__half2*>(my_row + (jj >> 3) * A_TILE_BYTES + (((jj & 7) ^ sw) << 4));
-          if (P.has_residual) {
-            const float2 f = __half22float2(*sp);
-            v0 += f.x; v1 += f.y;
+          for (int jj = 0; jj < BLOCK_N / 8; ++jj) {
+            const int cb = jj * 8 + (lane & 3) * 2;
+            float v0 = acc[m][4 * jj + 2 * h], v1 = acc[m][4 * jj + 2 * h + 1];
+            if (bias_row) { v0 += __ldg(bias_row + cb); v1 += __ldg(bias_row + cb + 1); }
+            if (temb_row) { v0 += __ldg(temb_row + cb); v1 += __ldg(temb_row + cb + 1); }
+            const int u = (jj & 3) * 2 + ((lane & 3) >> 1);
+            float2* sp = reinterpret_cast<float2*>(my_row + (jj >> 2) * A_TILE_BYTES + ((u ^ sw) << 4));
+            if (P.has_residual) {                  // the fp32 residual, never through a TF32 operand
+              const float2 f = *sp;
+              v0 += f.x; v1 += f.y;
+            }
+            *sp = make_float2(v0 * P.scale, v1 * P.scale);
           }
-          *sp = __floats2half2_rn(v0 * P.scale, v1 * P.scale);
+        } else {
+          uint8_t* my_row = staging + row * 128 + (lane & 3) * 4;
+          const int sw = row & 7;
+#pragma unroll
+          for (int jj = 0; jj < BLOCK_N / 8; ++jj) {
+            const int cb = jj * 8 + (lane & 3) * 2;  // channel inside the tile
+            float v0 = acc[m][4 * jj + 2 * h], v1 = acc[m][4 * jj + 2 * h + 1];
+            if (bias_row) { v0 += __ldg(bias_row + cb); v1 += __ldg(bias_row + cb + 1); }
+            if (temb_row) { v0 += __ldg(temb_row + cb); v1 += __ldg(temb_row + cb + 1); }
+            __half2* sp = reinterpret_cast<__half2*>(my_row + (jj >> 3) * A_TILE_BYTES + (((jj & 7) ^ sw) << 4));
+            if (P.has_residual) {
+              const float2 f = __half22float2(*sp);
+              v0 += f.x; v1 += f.y;
+            }
+            *sp = __floats2half2_rn(v0 * P.scale, v1 * P.scale);
+          }
         }
       }
     }
@@ -342,26 +388,42 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap map_a0, const __grid_constant
     if (wt == 0) {
 #pragma unroll
       for (int c = 0; c < L::N_CHUNKS; ++c)
-        tma_store_4d(&map_d, staging + c * A_TILE_BYTES, c_tile + c * 64, x0, y0, n0);
+        tma_store_4d(&map_d, staging + c * A_TILE_BYTES, c_tile + c * BK, x0, y0, n0);
       tma_store_commit();
     }
 
     if (P.stats) {
-      // per-channel (sum, sum^2) over each 32-row segment (one per warp), from the fp16 values actually stored
+      // per-channel (sum, sum^2) over each 32-row segment (one per warp), from the fp16 (fp32) values actually stored
       const int seg = wt >> 5;
+      if (TF32) {                 // (a plain if folds the same; it keeps the fp16 instantiations' SASS unchanged)
 #pragma unroll
-      for (int c = 0; c < L::N_CHUNKS; ++c) {
-        float s0 = 0.f, q0 = 0.f, s1 = 0.f, q1 = 0.f;
-        const uint8_t* cbase = staging + c * A_TILE_BYTES;
+        for (int c = 0; c < L::N_CHUNKS; ++c) {                // lane = channel of the 32-channel chunk
+          float s0 = 0.f, q0 = 0.f;
+          const uint8_t* cbase = staging + c * A_TILE_BYTES;
 #pragma unroll 8
-        for (int rr = 0; rr < 32; ++rr) {
-          const int r2 = seg * 32 + rr;
-          const __half2 hv = *reinterpret_cast<const __half2*>(cbase + r2 * 128 + ((((lane >> 2) ^ (r2 & 7)) << 4) | ((lane & 3) << 2)));
-          const float2 f = __half22float2(hv);
-          s0 += f.x; q0 += f.x * f.x; s1 += f.y; q1 += f.y * f.y;
+          for (int rr = 0; rr < 32; ++rr) {
+            const int r2 = seg * 32 + rr;
+            const float f = *reinterpret_cast<const float*>(cbase + r2 * 128 + ((((lane >> 2) ^ (r2 & 7)) << 4) | ((lane & 3) << 2)));
+            s0 += f; q0 += f * f;
+          }
+          float* d = stats_sm + ((seg * BLOCK_N) + c * 32 + lane) * 2;
+          d[0] = s0; d[1] = q0;
         }
-        float* d = stats_sm + ((seg * BLOCK_N) + c * 64 + lane * 2) * 2;
-        d[0] = s0; d[1] = q0; d[2] = s1; d[3] = q1;
+      } else {
+#pragma unroll
+        for (int c = 0; c < L::N_CHUNKS; ++c) {
+          float s0 = 0.f, q0 = 0.f, s1 = 0.f, q1 = 0.f;
+          const uint8_t* cbase = staging + c * A_TILE_BYTES;
+#pragma unroll 8
+          for (int rr = 0; rr < 32; ++rr) {
+            const int r2 = seg * 32 + rr;
+            const __half2 hv = *reinterpret_cast<const __half2*>(cbase + r2 * 128 + ((((lane >> 2) ^ (r2 & 7)) << 4) | ((lane & 3) << 2)));
+            const float2 f = __half22float2(hv);
+            s0 += f.x; q0 += f.x * f.x; s1 += f.y; q1 += f.y * f.y;
+          }
+          float* d = stats_sm + ((seg * BLOCK_N) + c * 64 + lane * 2) * 2;
+          d[0] = s0; d[1] = q0; d[2] = s1; d[3] = q1;
+        }
       }
       named_bar_sync(epi_bar, 128);
       const int groups = rps >= 128 ? 1 : 128 / rps;       // samples covered by this tile
@@ -408,27 +470,30 @@ EncodeTiledFn get_encode() {
   return fn;
 }
 
-// NHWC fp16 tensor, box {64 channels, bw, bh, bn}
-CUtensorMap make_act_map(const void* p, int N, int H, int W, int C, int bw, int bh, int bn) {
+// NHWC fp16 (esize 2) or fp32 (esize 4) tensor, box {one 128 B row of channels, bw, bh, bn}
+CUtensorMap make_act_map(const void* p, int N, int H, int W, int C, int bw, int bh, int bn, int esize = 2) {
   CUtensorMap m;
+  const cuuint64_t es_b = (cuuint64_t)esize;
   cuuint64_t dims[4] = {(cuuint64_t)C, (cuuint64_t)W, (cuuint64_t)H, (cuuint64_t)N};
-  cuuint64_t strides[3] = {(cuuint64_t)C * 2, (cuuint64_t)W * C * 2, (cuuint64_t)H * W * C * 2};
-  cuuint32_t box[4] = {64, (cuuint32_t)bw, (cuuint32_t)bh, (cuuint32_t)bn};
+  cuuint64_t strides[3] = {(cuuint64_t)C * es_b, (cuuint64_t)W * C * es_b, (cuuint64_t)H * W * C * es_b};
+  cuuint32_t box[4] = {(cuuint32_t)(ROW_BYTES / esize), (cuuint32_t)bw, (cuuint32_t)bh, (cuuint32_t)bn};
   cuuint32_t es[4] = {1, 1, 1, 1};
-  CUresult r = get_encode()(&m, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 4, const_cast<void*>(p), dims, strides, box, es,
+  const CUtensorMapDataType dt = esize == 4 ? CU_TENSOR_MAP_DATA_TYPE_FLOAT32 : CU_TENSOR_MAP_DATA_TYPE_FLOAT16;
+  CUresult r = get_encode()(&m, dt, 4, const_cast<void*>(p), dims, strides, box, es,
                             CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B,
                             CU_TENSOR_MAP_L2_PROMOTION_L2_128B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
   SG_CHECK(r == CUDA_SUCCESS, "cuTensorMapEncodeTiled(activation %dx%dx%dx%d box %dx%dx%d) failed: %d", N, H, W, C, bw, bh, bn, (int)r);
   return m;
 }
-// weights [Cout][Ktot] fp16, box {64, block_n}
-CUtensorMap make_w_map(const void* p, int Cout, int Ktot, int block_n) {
+// weights [Cout][Ktot] fp16 (esize 2) or TF32-valued fp32 (esize 4), box {one 128 B row of K, block_n}
+CUtensorMap make_w_map(const void* p, int Cout, int Ktot, int block_n, int esize = 2) {
   CUtensorMap m;
   cuuint64_t dims[2] = {(cuuint64_t)Ktot, (cuuint64_t)Cout};
-  cuuint64_t strides[1] = {(cuuint64_t)Ktot * 2};
-  cuuint32_t box[2] = {64, (cuuint32_t)block_n};
+  cuuint64_t strides[1] = {(cuuint64_t)Ktot * esize};
+  cuuint32_t box[2] = {(cuuint32_t)(ROW_BYTES / esize), (cuuint32_t)block_n};
   cuuint32_t es[2] = {1, 1};
-  CUresult r = get_encode()(&m, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 2, const_cast<void*>(p), dims, strides, box, es,
+  const CUtensorMapDataType dt = esize == 4 ? CU_TENSOR_MAP_DATA_TYPE_FLOAT32 : CU_TENSOR_MAP_DATA_TYPE_FLOAT16;
+  CUresult r = get_encode()(&m, dt, 2, const_cast<void*>(p), dims, strides, box, es,
                             CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B,
                             CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
   SG_CHECK(r == CUDA_SUCCESS, "cuTensorMapEncodeTiled(weights %dx%d) failed: %d", Cout, Ktot, (int)r);
@@ -465,10 +530,11 @@ TcPlan conv_tc_plan(const TensorDesc& out, int sms, bool narrow) {
   if (!choose_box(out.H, out.W, p.bw, p.bh, p.bn)) return TcPlan{};
   const int m_tiles = (out.W / p.bw) * (out.H / p.bh) * cdiv(out.N, p.bn);
   // tc1_narrow: when 128-wide channel tiles would fill less than half the SMs, 64-wide tiles double the CTAs.  The
-  // accumulation order of an output element does not depend on the tile width: bit-identical.
-  const bool wide = out.C % 128 == 0 && !(narrow && m_tiles * (out.C / 128) * 2 <= sms);
+  // accumulation order of an output element does not depend on the tile width: bit-identical.  fp32 (TF32) tiles are
+  // always 64 wide: their staging takes twice the bytes.
+  const bool wide = out.dt == DT_F16 && out.C % 128 == 0 && !(narrow && m_tiles * (out.C / 128) * 2 <= sms);
   p.block_n = wide ? 128 : 64;
-  p.stages = wide ? STAGES_N128 : STAGES_N64;
+  p.stages = out.dt == DT_F32 ? STAGES_TF32 : (wide ? STAGES_N128 : STAGES_N64);
   p.tiles = m_tiles * (out.C / p.block_n);
   p.grid = p.tiles < sms ? p.tiles : sms;
   if (p.grid > 0) { p.min_local = p.tiles / p.grid; p.max_local = cdiv(p.tiles, p.grid); }
@@ -477,9 +543,10 @@ TcPlan conv_tc_plan(const TensorDesc& out, int sms, bool narrow) {
 
 namespace {
 
-template <int BLOCK_N, int NUM_STAGES, bool FUSED>
+template <int BLOCK_N, int NUM_STAGES, bool FUSED, typename T>
 void launch_impl(cudaStream_t st, const ConvArgs& a, TensorDesc& out, int* dbg, const TcPlan& plan) {
-  using L = SmemLayout<BLOCK_N, NUM_STAGES>;
+  using L = SmemLayout<BLOCK_N, NUM_STAGES, sizeof(T)>;
+  constexpr int ES = sizeof(T), BK = kBlockK<T>;
   const int bw = plan.bw, bh = plan.bh, bn = plan.bn;
   TcParams P{};
   P.bw = bw; P.bh = bh; P.bn = bn;
@@ -493,11 +560,11 @@ void launch_impl(cudaStream_t st, const ConvArgs& a, TensorDesc& out, int* dbg, 
   int kblocks = 0;
   for (int i = 0; i < 3; ++i) {
     const TensorDesc& s = a.seg[i < a.nseg ? i : 0].src;
-    ma[i] = make_act_map(s.p, s.N, s.H, s.W, s.C, bw, bh, bn);
+    ma[i] = make_act_map(s.p, s.N, s.H, s.W, s.C, bw, bh, bn, ES);
     if (i < a.nseg) {
       const int cin = s.C + (i == 0 && FUSED && a.gn_has_cat ? a.gn_cat.C : 0);
-      P.seg_chunks[i] = cin / 64; P.seg_taps[i] = a.seg[i].taps;
-      kblocks += a.seg[i].taps * (cin / 64);
+      P.seg_chunks[i] = cin / BK; P.seg_taps[i] = a.seg[i].taps;
+      kblocks += a.seg[i].taps * (cin / BK);
     }
   }
   P.num_k_blocks = kblocks;
@@ -506,17 +573,17 @@ void launch_impl(cudaStream_t st, const ConvArgs& a, TensorDesc& out, int* dbg, 
     P.raw1 = a.gn_has_cat ? static_cast<const __half*>(a.gn_cat.p) : nullptr; P.c1 = a.gn_has_cat ? a.gn_cat.C : 0;
     P.gn_ab = a.gn_ab;
   }
-  const CUtensorMap mb = make_w_map(a.w_tc, out.C, a.w_tc_ld ? a.w_tc_ld : a.ktot(), BLOCK_N);
-  const CUtensorMap md = make_act_map(out.p, out.N, out.H, out.W, out.C, bw, bh, bn);
+  const CUtensorMap mb = make_w_map(a.w_tc, out.C, a.w_tc_ld ? a.w_tc_ld : a.ktot(), BLOCK_N, ES);
+  const CUtensorMap md = make_act_map(out.p, out.N, out.H, out.W, out.C, bw, bh, bn, ES);
   const TensorDesc& rs = a.residual ? *a.residual : out;
-  const CUtensorMap mr = make_act_map(rs.p, rs.N, rs.H, rs.W, rs.C, bw, bh, bn);
+  const CUtensorMap mr = make_act_map(rs.p, rs.N, rs.H, rs.W, rs.C, bw, bh, bn, ES);
   P.bias = a.bias; P.temb = a.temb; P.temb_stride = a.temb_stride;
   P.has_residual = a.residual ? 1 : 0;
   P.scale = a.scale;
   out.slots = P.tiles_w * P.tiles_h;
   P.stats = out.stats; P.slots = out.slots;
   P.dbg = dbg;
-  auto kern = conv_tc_kernel<BLOCK_N, NUM_STAGES, FUSED>;
+  auto kern = conv_tc_kernel<BLOCK_N, NUM_STAGES, FUSED, T>;
   static unsigned long long attr_devs = 0;
   if (first_use_on_device(attr_devs)) {
     CUDA_OK(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, L::DYN_BYTES));
@@ -529,8 +596,15 @@ template <bool FUSED>
 void launch_width(cudaStream_t st, const ConvArgs& a, TensorDesc& out, int* dbg) {
   const TcPlan plan = conv_tc_plan(out, num_sms(), g_tc1_narrow != 0);
   SG_CHECK(plan.bw > 0, "conv_tc: no 128-pixel box for %dx%d", out.H, out.W);
-  if (plan.block_n == 128) launch_impl<128, STAGES_N128, FUSED>(st, a, out, dbg, plan);
-  else launch_impl<64, STAGES_N64, FUSED>(st, a, out, dbg, plan);
+  if (plan.block_n == 128) launch_impl<128, STAGES_N128, FUSED, __half>(st, a, out, dbg, plan);
+  else launch_impl<64, STAGES_N64, FUSED, __half>(st, a, out, dbg, plan);
+}
+
+// fp32 activations, TF32 operands: one tile width and ring depth (conv_tc_plan)
+void launch_tf32(cudaStream_t st, const ConvArgs& a, TensorDesc& out, int* dbg) {
+  const TcPlan plan = conv_tc_plan(out, num_sms(), false);
+  SG_CHECK(plan.bw > 0, "conv_tc: no 128-pixel box for %dx%d", out.H, out.W);
+  launch_impl<64, STAGES_TF32, false, float>(st, a, out, dbg, plan);
 }
 
 }  // namespace
@@ -540,9 +614,10 @@ thread_local int g_tc1_narrow = 0;   // see launch_width
 volatile int* g_wait_code_host = nullptr;
 
 bool conv_tc_supported(const ConvArgs& a, const TensorDesc& out) {
-  if (out.dt != DT_F16 || out.C % 64 != 0 || a.w_tc == nullptr) return false;
+  if (out.C % 64 != 0 || a.w_tc == nullptr) return false;
+  const int ck = out.dt == DT_F16 ? 64 : 32;        // channels of one k-block
   for (int i = 0; i < a.nseg; ++i)
-    if (a.seg[i].src.C % 64 != 0 || a.seg[i].src.dt != DT_F16) return false;
+    if (a.seg[i].src.C % ck != 0 || a.seg[i].src.dt != out.dt) return false;
   int bw, bh, bn;
   return choose_box(out.H, out.W, bw, bh, bn);
 }
@@ -559,7 +634,12 @@ void launch_conv_tc(cudaStream_t st, const ConvArgs& a, TensorDesc& out, int* db
     const TensorDesc& s = a.seg[i].src;
     SG_CHECK(s.N == out.N && s.H == out.H && s.W == out.W, "conv_tc: segment %d shape mismatch", i);
   }
-  if (a.residual) SG_CHECK(a.residual->C == out.C && a.residual->dt == DT_F16, "conv_tc: residual mismatch");
+  if (a.residual) SG_CHECK(a.residual->C == out.C && a.residual->dt == out.dt, "conv_tc: residual mismatch");
+  if (out.dt == DT_F32) {
+    SG_CHECK(a.gn_ab == nullptr, "conv_tc: the fused GroupNorm producer is fp16 only");
+    launch_tf32(st, a, out, dbg);
+    return;
+  }
   if (a.gn_ab) {                                                      // the engine only asks for fusion when it applies
     SG_CHECK(a.seg[0].taps == 9 && conv_tc_fuse_shape_ok(out.H, out.W, a.seg[0].src.C, a.gn_has_cat ? a.gn_cat.C : 0, out.C) &&
                  (!a.gn_has_cat || (a.gn_cat.dt == DT_F16 && a.gn_cat.N == out.N && a.gn_cat.H == out.H && a.gn_cat.W == out.W)),

@@ -160,6 +160,13 @@ template <typename T> T from_float(float v);
 template <> float from_float<float>(float v) { return v; }
 template <> __half from_float<__half>(float v) { return __float2half_rn(v); }
 
+// activation element type of the mode: fp32 in fp32 and tf32_tc, fp16 otherwise
+DType act_dtype(const sgmse_b200_config& c) {
+  return c.mode == SGMSE_B200_MODE_FP32 || c.mode == SGMSE_B200_MODE_TF32_TC ? DT_F32 : DT_F16;
+}
+// the modes whose convolutions run on the wgmma kernel where it tiles the shape
+bool tc_mode(const sgmse_b200_config& c) { return c.mode == SGMSE_B200_MODE_FP16_TC || c.mode == SGMSE_B200_MODE_TF32_TC; }
+
 void* upload(Engine& e, const void* host, size_t bytes) {
   void* d = nullptr;
   CUDA_OK(cudaMalloc(&d, bytes));
@@ -190,9 +197,18 @@ void pack_conv(Engine& e, const std::vector<PackSrc>& srcs, int cout, bool out_m
       }
     kbase += s.taps * s.cin;
   }
-  const bool f16 = e.cfg.mode != SGMSE_B200_MODE_FP32;
+  const bool f16 = act_dtype(e.cfg) == DT_F16;
   if (!f16) {
     cw.w_direct = upload(e, kd.data(), kd.size() * 4);
+    if (e.cfg.mode == SGMSE_B200_MODE_TF32_TC && cout % 64 == 0 && ktot % 32 == 0) {
+      // [Cout][ktot] TF32 values (round to nearest, ties away); no identity tail: the residual stays out of the TF32
+      // operands and is added in fp32 by the epilogue
+      std::vector<float> ht((size_t)cout * ktot);
+      for (int k = 0; k < ktot; ++k)
+        for (int co = 0; co < cout; ++co) ht[(size_t)co * ktot + k] = tf32_rna(kd[(size_t)k * cout + co]);
+      cw.w_tc = upload(e, ht.data(), ht.size() * 4);
+      cw.w_tc_ld = ktot;
+    }
   } else {
     std::vector<__half> hd(kd.size());
     for (size_t i = 0; i < kd.size(); ++i) hd[i] = __float2half_rn(kd[i]);
@@ -207,7 +223,7 @@ void pack_conv(Engine& e, const std::vector<PackSrc>& srcs, int cout, bool out_m
         for (int co = 0; co < cout; ++co) ht[(size_t)co * ld + k] = hd[(size_t)k * cout + co];
       if (identity_tail)
         for (int co = 0; co < cout; ++co) ht[(size_t)co * ld + ktot + co] = __float2half_rn(1.f);
-      cw.w_tc = (__half*)upload(e, ht.data(), ht.size() * 2);
+      cw.w_tc = upload(e, ht.data(), ht.size() * 2);
       cw.w_tc_ld = ld;
       cw.identity_tail = identity_tail;
     }
@@ -360,7 +376,7 @@ void* dev_alloc(Engine& e, size_t bytes) {
 }
 void pack_conv_dev(Engine& e, cudaStream_t st, const PackJob& job_in, ConvW& cw) {
   PackJob j = job_in;
-  const bool f16 = e.cfg.mode != SGMSE_B200_MODE_FP32;
+  const bool f16 = act_dtype(e.cfg) == DT_F16;
   cw.ktot = j.ktot; cw.cout = j.cout;
   const size_t n = (size_t)j.ktot * j.cout;
   cw.w_direct = dev_alloc(e, n * (f16 ? 2 : 4));
@@ -372,6 +388,11 @@ void pack_conv_dev(Engine& e, cudaStream_t st, const PackJob& job_in, ConvW& cw)
     cw.w_tc = ht; cw.w_tc_ld = j.ld; cw.identity_tail = j.identity_tail != 0;
   }
   launch_pack_conv(st, e.blob_dev, j, cw.w_direct, f16, ht);
+  if (e.cfg.mode == SGMSE_B200_MODE_TF32_TC && j.cout % 64 == 0 && j.ktot % 32 == 0) {   // as pack_conv: no identity tail
+    cw.w_tc = dev_alloc(e, n * 4);
+    cw.w_tc_ld = j.ktot;
+    launch_pack_tc_tf32(st, (const float*)cw.w_direct, j.ktot, j.cout, j.ktot, (float*)cw.w_tc);
+  }
 }
 PackJob conv_job(std::initializer_list<PackSeg> segs, int cout, int mode, bool identity_tail) {
   PackJob j{};
@@ -491,7 +512,7 @@ struct Fwd {
 
   void conv(const ConvArgs& a, TensorDesc& out, int cls) {
     if (dry) return;
-    const bool want_tc = e.cfg.mode == SGMSE_B200_MODE_FP16_TC && ((e.tc_mask >> cls) & 1);
+    const bool want_tc = tc_mode(e.cfg) && ((e.tc_mask >> cls) & 1);
     const bool tc = a.gn_ab != nullptr || (want_tc && conv_tc_supported(a, out));
     cudaEvent_t ev0 = nullptr, ev1 = nullptr;
     if (e.time_convs) {
@@ -791,7 +812,7 @@ void ensure_arena(Engine& e, int B, int F, int T) {
     Arena saved = e.arena;
     e.arena = Arena{};
     e.arena.dry = true;
-    Fwd f{e, nullptr, nullptr, 0, true, e.cfg.mode == SGMSE_B200_MODE_FP32 ? DT_F32 : DT_F16};
+    Fwd f{e, nullptr, nullptr, 0, true, act_dtype(e.cfg)};
     f.run(nullptr, B, F, T);
     const size_t need = e.arena.high + 4096;
     e.arena = saved;
@@ -872,7 +893,7 @@ void dnn_forward(Engine& e, const float2* x, const float2* y, const float* t, fl
     const int Bc = std::min(mb, B - b0);
     launch_pack_state(st, x + b0 * px1, y + b0 * px1, Bc, F, T, e.state); ++e.kernel_launches;
     launch_temb(st, temb_weights(e), t + b0, Bc, e.temb_scratch, e.temb_table); e.kernel_launches += 2;
-    Fwd f{e, st, e.temb_table, e.total_temb_c, false, e.cfg.mode == SGMSE_B200_MODE_FP32 ? DT_F32 : DT_F16};
+    Fwd f{e, st, e.temb_table, e.total_temb_c, false, act_dtype(e.cfg)};
     const float4* p = f.run(e.state, Bc, F, T);
     launch_out_layer(st, p, Bc, F, T, e.out_layer, t + b0, out + b0 * px1, negate); ++e.kernel_launches;
   }
@@ -1049,7 +1070,7 @@ void sample_chunk(Engine& e, const float2* y, int Bc, int F, int T, const sgmse_
       launch_prior(st, e.state, Bc, F, T, (float)ouve_std(c, 1.0), nz(draw), rng, draw); ++e.kernel_launches;
       ++draw;
     }
-    Fwd f{e, st, nullptr, 0, false, e.cfg.mode == SGMSE_B200_MODE_FP32 ? DT_F32 : DT_F16};
+    Fwd f{e, st, nullptr, 0, false, act_dtype(e.cfg)};
     bool have_mean = false;
     for (int i = 0; i < s.N; ++i) {
       f.temb = e.temb_table + (size_t)i * e.total_temb_c;
@@ -1085,7 +1106,7 @@ void sample_chunk(Engine& e, const float2* y, int Bc, int F, int T, const sgmse_
   ++draw;
   int ci = 0;
   bool have_mean = false;
-  Fwd f{e, st, nullptr, 0, false, e.cfg.mode == SGMSE_B200_MODE_FP32 ? DT_F32 : DT_F16};
+  Fwd f{e, st, nullptr, 0, false, act_dtype(e.cfg)};
   for (int i = 0; i < s.N; ++i) {
     const float inv_t = 1.0f / tb.ts[i];
     f.temb = e.temb_table + (size_t)i * e.total_temb_c;
@@ -1204,7 +1225,7 @@ void pc_sample(Engine& e, const float2* y, int B, int F, int T, const sgmse_b200
       // one eager network evaluation first: sets function attributes and surfaces launch errors early
       {
         launch_pack_state(st, y + b0 * px1, y + b0 * px1, ln[0], F, T, e.state);
-        Fwd f{e, st, e.temb_table, 0, false, e.cfg.mode == SGMSE_B200_MODE_FP32 ? DT_F32 : DT_F16};
+        Fwd f{e, st, e.temb_table, 0, false, act_dtype(e.cfg)};
         f.run(e.state, ln[0], F, T);
         CUDA_OK(cudaStreamSynchronize(st));
       }
@@ -1286,7 +1307,7 @@ void ensure_ode(Engine& e, size_t px) {
 // solve is hundreds of evaluations of the same sequence with nothing but t changing, and t lives in device memory
 // (temb row, drift coefficients are kernel arguments of the un-captured drift kernel).
 const float4* forward_on_state(Engine& e, int Bc, int F, int T, cudaStream_t st, float in_scale = 1.f) {
-  Fwd f{e, st, e.temb_table, 0, false, e.cfg.mode == SGMSE_B200_MODE_FP32 ? DT_F32 : DT_F16};
+  Fwd f{e, st, e.temb_table, 0, false, act_dtype(e.cfg)};
   f.in_scale = in_scale;                                       // c_in(t) of a preconditioned model: a kernel argument, so
   const bool graph_ok = e.cfg.use_graphs && !e.time_convs && !e.record_taps && st != nullptr && in_scale == 1.f;   // not graphed
   if (!graph_ok) return f.run(e.state, Bc, F, T);
@@ -1538,7 +1559,7 @@ void check_range(Engine& e, cudaStream_t st) {
   if (v) {
     CUDA_OK(cudaMemsetAsync(e.range_flag, 0, sizeof(unsigned int), st));
     SG_CHECK(false, "fp16 activation range exceeded: %u GroupNorm input group(s) held values beyond +-65504 (stored as inf); "
-                    "the result is not usable -- run this model in mode fp32", v);
+                    "the result is not usable -- run this model in mode tf32_tc (fp32 activations on tensor cores)", v);
   }
 }
 
@@ -1647,7 +1668,7 @@ int sgmse_b200_create(const sgmse_b200_config* cfg, sgmse_b200_engine** out) {
   std::unique_ptr<Engine> e(new Engine());
   e->cfg = *cfg;
   if (e->cfg.max_batch <= 0) e->cfg.max_batch = 8;
-  SG_CHECK(cfg->mode >= 0 && cfg->mode <= 2, "unknown mode %d", cfg->mode);
+  SG_CHECK(cfg->mode >= 0 && cfg->mode <= 3, "unknown mode %d", cfg->mode);
   build_network(*e);                          // host only: no CUDA call before the first weights arrive
   *out = e.release();
   API_END
@@ -1750,7 +1771,7 @@ int sgmse_b200_model_forward(sgmse_b200_engine* e, const void* x_t, const void* 
       launch_pack_state_scaled(st, (const float2*)x_t + b0 * px1, (const float2*)y + b0 * px1, vec, Bc, F, T, e->state);
       ++e->kernel_launches;
       launch_temb(st, temb_weights(*e), t + b0, Bc, e->temb_scratch, e->temb_table); e->kernel_launches += 2;
-      Fwd f{*e, st, e->temb_table, e->total_temb_c, false, e->cfg.mode == SGMSE_B200_MODE_FP32 ? DT_F32 : DT_F16};
+      Fwd f{*e, st, e->temb_table, e->total_temb_c, false, act_dtype(e->cfg)};
       const float4* p = f.run(e->state, Bc, F, T);
       launch_precond_out(st, (const float2*)x_t + b0 * px1, p, Bc, F, T, e->out_layer, vec + Bc, vec + 2 * Bc,
                          (float2*)out + b0 * px1);
@@ -1910,7 +1931,7 @@ long long sgmse_b200_workspace_bytes(sgmse_b200_engine* e, int B, int F, int T) 
     Arena saved = e->arena;
     e->arena = Arena{};
     e->arena.dry = true;
-    Fwd f{*e, nullptr, nullptr, 0, true, e->cfg.mode == SGMSE_B200_MODE_FP32 ? DT_F32 : DT_F16};
+    Fwd f{*e, nullptr, nullptr, 0, true, act_dtype(e->cfg)};
     try { f.run(nullptr, B, F, T); } catch (...) { e->arena = saved; throw; }
     const long long need = (long long)e->arena.high + 4096;
     e->arena = saved;

@@ -21,7 +21,7 @@ struct ParamRef {       // one state_dict() entry
 
 struct ConvW {          // packed convolution weights (K ordering: segment, tap, cin)
   void* w_direct = nullptr;   // [Ktot][Cout] float or half
-  __half* w_tc = nullptr;     // [Cout][w_tc_ld], K-major; optional identity tail (see pack_conv)
+  void* w_tc = nullptr;       // [Cout][w_tc_ld], K-major: fp16 (optional identity tail, see pack_conv) or TF32-valued fp32
   int w_tc_ld = 0;
   bool identity_tail = false;
   float* bias = nullptr;      // [Cout] fp32 (device)

@@ -3,6 +3,7 @@
 // partial (sum, sum of squares) written by the producer of a tensor and consumed by gn_finalize.
 #pragma once
 #include <algorithm>
+#include <cstring>
 
 #include "common.cuh"
 
@@ -51,7 +52,7 @@ struct ConvArgs {
   int nseg = 0;
   ConvSeg seg[3];
   const void* w_direct = nullptr;  // [Ktot][Cout], element type of the activations
-  const __half* w_tc = nullptr;    // [Cout][w_tc_ld] (K-major rows)
+  const void* w_tc = nullptr;      // [Cout][w_tc_ld] (K-major rows): fp16, or fp32 holding TF32 values (tf32_rna) for fp32 activations
   int w_tc_ld = 0;                 // row length in elements (>= ktot())
   bool tc_identity_tail = false;   // columns [ktot, ktot+Cout) hold I: the residual may be fed as a K segment
   const float* bias = nullptr;     // [Cout] (nullable)
@@ -71,7 +72,8 @@ struct ConvArgs {
   }
 };
 void launch_conv_direct(cudaStream_t st, const ConvArgs& a, TensorDesc& out);
-// wgmma implicit GEMM (conv_tc.cu); requires fp16 activations, every segment C % 64 == 0, Cout % 64 == 0
+// wgmma implicit GEMM (conv_tc.cu); requires Cout % 64 == 0 and either fp16 activations with every segment C % 64 == 0, or
+// fp32 activations (TF32 operands) with every segment C % 32 == 0
 bool conv_tc_supported(const ConvArgs& a, const TensorDesc& out);
 // shape test of the fused GroupNorm-apply/SiLU form (3x3 over c0 [+ c1] raw channels), usable before the tensors exist
 bool conv_tc_fuse_shape_ok(int H, int W, int c0, int c1, int cout);
@@ -212,6 +214,17 @@ void launch_overlap_add(cudaStream_t st, const float* frames, const float* norm,
 struct PackSeg { long long w; int cin, taps, kbase; };
 struct PackJob { PackSeg seg[4]; int nseg, cout, ktot, ld, mode, identity_tail; };
 void launch_pack_conv(cudaStream_t st, const float* blob, const PackJob& j, void* kd, bool kd_half, __half* ht);
+// conv_tc's TF32 weight operand: wt[co][ld] = tf32_rna(kd[k][co]) for k < ktot, from the fp32 [ktot][cout] direct layout
+void launch_pack_tc_tf32(cudaStream_t st, const float* kd, int ktot, int cout, int ld, float* wt);
+// fp32 -> the nearest TF32 value (10 mantissa bits), ties away from zero (the rounding of cvt.rna.tf32.f32); the same
+// integer arithmetic on host and device, so both weight packers agree bit for bit
+__host__ __device__ inline float tf32_rna(float v) {
+  uint32_t u;
+  memcpy(&u, &v, 4);
+  if ((u & 0x7F800000u) != 0x7F800000u) u = (u + 0x1000u) & 0xFFFFE000u;   // Inf and NaN pass through
+  memcpy(&v, &u, 4);
+  return v;
+}
 void launch_pack_inconv(cudaStream_t st, const float* w, int nf, float* out);
 void launch_pack_combine(cudaStream_t st, const float* w, int C, float* out);
 void launch_pack_outconv(cudaStream_t st, const float* w, int C, float* out, uint2* frag);

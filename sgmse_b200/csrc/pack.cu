@@ -7,7 +7,8 @@
 
 namespace sgmse {
 
-// [k][cout] (fp32 or fp16) and, optionally, [cout][ld] fp16 (K-major, conv_tc) of up to four K segments.
+// [k][cout] (fp32 or fp16) and, optionally, [cout][ld] fp16 (K-major, conv_tc) of up to four K segments.  (The TF32 operand
+// of the fp32 activations is transposed from the fp32 [k][cout] result by pack_tc_tf32_kernel.)
 //   mode 0: Conv2d weights [cout][cin][taps];  mode 1: NIN weights [cin][cout];
 //   mode 2: three NIN weights [cin][cout/3] side by side (q | k | v of the attention block; seg[0..2].w hold the three offsets)
 template <typename T>
@@ -35,6 +36,13 @@ __global__ void identity_tail_kernel(__half* __restrict__ ht, int cout, int ld, 
   if (idx >= cout * cout) return;
   const int co = idx / cout, c2 = idx - co * cout;
   ht[(long long)co * ld + ktot + c2] = __float2half_rn(co == c2 ? 1.f : 0.f);
+}
+// [ktot][cout] fp32 -> [cout][ld] TF32 values (conv_tc's K-major B operand for fp32 activations); ld == ktot: no identity tail
+__global__ void pack_tc_tf32_kernel(const float* __restrict__ kd, int ktot, int cout, int ld, float* __restrict__ wt) {
+  const long long idx = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+  if (idx >= (long long)ktot * cout) return;
+  const int k = (int)(idx / cout), co = (int)(idx - (long long)k * cout);
+  wt[(long long)co * ld + k] = tf32_rna(kd[idx]);
 }
 // input conv [nf][4][3][3] -> [36][nf]
 __global__ void pack_inconv_kernel(const float* __restrict__ w, int nf, float* __restrict__ out) {
@@ -88,6 +96,10 @@ void launch_pack_conv(cudaStream_t st, const float* blob, const PackJob& j, void
     identity_tail_kernel<<<blocks((long long)j.cout * j.cout), 256, 0, st>>>(ht, j.cout, j.ld, j.ktot);
     CUDA_OK(cudaGetLastError());
   }
+}
+void launch_pack_tc_tf32(cudaStream_t st, const float* kd, int ktot, int cout, int ld, float* wt) {
+  pack_tc_tf32_kernel<<<blocks((long long)ktot * cout), 256, 0, st>>>(kd, ktot, cout, ld, wt);
+  CUDA_OK(cudaGetLastError());
 }
 void launch_pack_inconv(cudaStream_t st, const float* w, int nf, float* out) {
   pack_inconv_kernel<<<blocks(36LL * nf), 256, 0, st>>>(w, nf, out);

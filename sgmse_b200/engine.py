@@ -15,7 +15,7 @@ import torch
 
 from . import _lib
 
-MODES = {"fp32": 0, "fp16_direct": 1, "fp16_tc": 2}
+MODES = {"fp32": 0, "fp16_direct": 1, "fp16_tc": 2, "tf32_tc": 3}
 PREDICTORS = {"reverse_diffusion": 0, "euler_maruyama": 1, "none": 2}
 CORRECTORS = {"ald": 0, "langevin": 1, "none": 2}
 PAD_MODES = {"zero_pad": 0, "reflection": 1}

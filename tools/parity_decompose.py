@@ -4,6 +4,7 @@ own CPU enhancement of one 4-s clip) repeated under engine modes / A-B options t
     python tools/parity_decompose.py            # on the GPU; prints one line per setting (SI-SDR / rel-L2 vs the reference)
 
 fp32            : CUDA-core validation mode (no approximation besides summation order)
+tf32_tc         : fp32 storage, wgmma convolutions with TF32 operands -> what 10-bit operands alone cost
 fp16_direct     : CUDA-core convolutions, fp16 STORAGE of activations, exact expf SiLU -> what storage alone costs
 fp16_tc         : the product mode (wgmma, fused GroupNorm+SiLU producers, fp16 FIR arithmetic, mma.sync ends)
 fp16_tc + opts  : tc_variant=5 (GroupNorm+SiLU fused into the convolutions), fir_variant=1 (fp32 FIR), inconv_variant=1 /
@@ -30,7 +31,7 @@ draws = o_sde.make_noise((1, 1, 256, 512), o_sde.n_noise_draws(N, "reverse_diffu
 noise = torch.stack(draws).cuda()
 ref = z["enh"]
 
-SETTINGS = [("fp32", {}), ("fp16_direct", {}), ("fp16_tc", {}), ("fp16_tc", {"tc_variant": 5}), ("fp16_tc", {"fir_variant": 1}),
+SETTINGS = [("fp32", {}), ("tf32_tc", {}), ("fp16_direct", {}), ("fp16_tc", {}), ("fp16_tc", {"tc_variant": 5}), ("fp16_tc", {"fir_variant": 1}),
             ("fp16_tc", {"inconv_variant": 1}), ("fp16_tc", {"outconv_variant": 1}),
             ("fp16_tc", {"fir_variant": 1, "inconv_variant": 1, "outconv_variant": 1})]
 outs = {}
