@@ -5,16 +5,24 @@
 //
 // GEMM view: M = N*H*W pixels (tiles of 128 = one TMA box bw x bh x bn of pixels), N = Cout (tiles of
 // BLOCK_N), K = sum over segments of taps*Cin (blocks of 64 channels of one tap).  There is no im2col
-// buffer: for each (tap, 64-channel chunk) the producer issues ONE 4-D TMA box load of the activation
-// tensor at the tap-shifted pixel coordinates; TMA zero-fills out-of-bounds pixels, which is exactly
-// the conv's zero padding, and lands the box as a 128-row K-major SWIZZLE_128B operand tile.  Several
-// K segments let one accumulator take  conv3x3(h) + conv1x1(x_a) + conv1x1(x_b)  (ResnetBlockBigGANpp's
-// Conv_1 plus the Conv_2 shortcut over a concatenated skip input) without materialising the concat.
+// buffer: the activations come in by 4-D TMA box loads at tap-shifted pixel coordinates; TMA zero-fills
+// out-of-bounds pixels, which is exactly the conv's zero padding, and lands each box as K-major
+// SWIZZLE_128B rows.  A 3x3 segment over a single-sample box with bw % 8 == 0 (tc_strip_rows,
+// conv_tc_sched.h) loads one dy-halo strip of bw x (bh + 2) pixels per (dx, 64-channel chunk): the
+// 128-row tiles of taps dy = -1, 0, +1 start 0, bw and 2 bw rows into it (whole 1024 B swizzle atoms),
+// so one load serves three k-blocks and the segment's A traffic falls from 9 to 3 (bh + 2) / bh boxes
+// per chunk.  Its k-blocks are issued dx-major (dx, chunk, dy), each against the weight column of its
+// tap.  Elsewhere (multi-sample boxes, bw = 4, 1x1 segments, the fused producer) each (tap, chunk) has
+// one 128-pixel box.  Several K segments let one accumulator take  conv3x3(h) + conv1x1(x_a) +
+// conv1x1(x_b)  (ResnetBlockBigGANpp's Conv_1 plus the Conv_2 shortcut over a concatenated skip input)
+// without materialising the concat.
 //
 // Persistent, warp-specialised CTA (384 threads = 3 warpgroups, 1 CTA/SM), "ping-pong" consumers:
-//   warpgroup 0   producer (register budget cut with setmaxnreg): one thread issues the TMA loads into an smem ring
-//                 of NUM_STAGES x {A 16 KB, B BLOCK_N*128 B}, in tile order.  With FUSED (GroupNorm-apply + SiLU of
-//                 the 3x3 input, see below) all 128 threads build the segment-0 A tiles from the RAW tensor instead.
+//   warpgroup 0   producer (register budget cut with setmaxnreg): one thread issues the TMA loads, in tile order,
+//                 into two mbarrier-guarded smem rings: B, NUM_STAGES weight tiles of BLOCK_N*128 B, one per
+//                 k-block; A, A_STAGES slots of 20 KB, one strip (three k-blocks) or one 16 KB box (one k-block)
+//                 each.  With FUSED (GroupNorm-apply + SiLU of the 3x3 input, see below) all 128 threads build the
+//                 segment-0 A tiles from the RAW tensor instead, one per k-block.
 //   warpgroups 1, 2   (register budget raised with setmaxnreg) each own every other tile of the CTA (local tiles
 //                 j & 1 == 0 and 1) and compute the whole 128-pixel tile: two wgmma m64nBLOCK_Nk16 per k16 step
 //                 (rows 0-63 and 64-127).  The MMA turn passes between them through a pair of named barriers once
@@ -28,9 +36,9 @@
 // (seg[0].src, concatenated with gn_cat), so the gn_apply pass and its buffer disappear.  Out-of-image taps read 0
 // (the padding of the ACTIVATED tensor, as in F.conv2d after the activation).
 //
-// TF32 (T = float, mode tf32_tc): the same ring, descriptors and schedule in bytes.  One 128 B swizzle row holds 32 fp32
-// channels, so a K block is 32 channels of one tap and a wgmma m64n64k8 TF32 step covers 8 (4 steps per block, +32 B each,
-// as for fp16).  The tensor cores read the upper 19 bits of each fp32 operand; the weights are stored RNA-rounded to TF32
+// TF32 (T = float, mode tf32_tc): the same rings, strips, descriptors and schedule in bytes.  One 128 B swizzle row holds
+// 32 fp32 channels, so a K block is 32 channels of one tap and a wgmma m64n64k8 TF32 step covers 8 (4 steps per block,
+// +32 B each, as for fp16).  The tensor cores read the upper 19 bits of each fp32 operand; the weights are stored RNA-rounded to TF32
 // (tf32_rna), the activations go in as stored.  The epilogue stages fp32 (32 channels per 128 B row), adds bias, time
 // embedding and the fp32 residual, and reduces the GroupNorm partials from the staged fp32 values.  Tiles are 64 channels
 // wide (fp32 staging is twice the bytes) and the fused GroupNorm producer is fp16 only.
@@ -67,6 +75,7 @@ struct TcParams {
   int seg_chunks[3];
   int seg_taps[3];
   int num_k_blocks;
+  int strip_chunks, strip_rows;   // segment 0 fed from dy-halo strips (conv_tc_sched.h): its chunks and strip rows; 0: boxes
   const float* bias;
   const float* temb;
   int temb_stride;
@@ -82,21 +91,31 @@ struct TcParams {
   int* dbg;
 };
 
+// A ring depth: as many 20 KB slots as the rest of each instantiation's budget leaves (checked in SmemLayout)
+constexpr int A_STAGES_N128 = 4, A_STAGES_N64 = 6, A_STAGES_TF32 = 5;
+
 template <int BLOCK_N, int NUM_STAGES, int ESIZE = 2>   // ESIZE: bytes per activation element (2 fp16, 4 fp32)
 struct SmemLayout {
   static constexpr int B_TILE_BYTES = BLOCK_N * ROW_BYTES;
-  static constexpr int STAGE_BYTES = A_TILE_BYTES + B_TILE_BYTES;
+  static constexpr int A_STAGES = ESIZE == 4 ? A_STAGES_TF32 : (BLOCK_N == 128 ? A_STAGES_N128 : A_STAGES_N64);
+  static constexpr int A_SLOT_BYTES = TC_STRIP_MAX_ROWS * ROW_BYTES;  // one strip (<= 20 KB) or one 16 KB box
   static constexpr int N_CHUNKS = BLOCK_N * ESIZE / ROW_BYTES;          // 128 B-row output chunks of the staged tile
   static constexpr int STAGING_BYTES = N_CHUNKS * A_TILE_BYTES;         // per consumer warpgroup
   static constexpr int STATS_BYTES = 4 * BLOCK_N * 2 * 4;               // per consumer warpgroup: float [4][BLOCK_N][2]
-  static constexpr int OFF_STAGING = NUM_STAGES * STAGE_BYTES;
+  static constexpr int OFF_A = NUM_STAGES * B_TILE_BYTES;               // the B ring starts at 0
+  static constexpr int OFF_STAGING = OFF_A + A_STAGES * A_SLOT_BYTES;
   static constexpr int OFF_STATS = OFF_STAGING + 2 * STAGING_BYTES;
   static constexpr int OFF_BARS = OFF_STATS + 2 * STATS_BYTES;
-  static constexpr int NUM_BARS = 2 * NUM_STAGES + 2;                   // full[], empty[], residual[2]
+  static constexpr int NUM_BARS = 2 * NUM_STAGES + 2 * A_STAGES + 2;    // B full[], empty[], A full[], empty[], residual[2]
   static constexpr int TOTAL = OFF_BARS + NUM_BARS * 8;
   static constexpr int DYN_BYTES = TOTAL + 1024;                        // slack for 1024 B alignment
+  static_assert(A_SLOT_BYTES % 1024 == 0 && OFF_A % 1024 == 0, "conv_tc: A slots must start on 1024 B swizzle atoms");
+  static_assert(A_STAGES >= 2, "conv_tc: a strip slot is released one k-block after its last use");
   static_assert(DYN_BYTES <= 227 * 1024, "conv_tc: shared memory over the sm_90 per-block limit");
 };
+static_assert(SmemLayout<128, STAGES_N128>::DYN_BYTES <= 227 * 1024, "conv_tc: 128-wide fp16 budget");
+static_assert(SmemLayout<64, STAGES_N64>::DYN_BYTES <= 227 * 1024, "conv_tc: 64-wide fp16 budget");
+static_assert(SmemLayout<64, STAGES_TF32, 4>::DYN_BYTES <= 227 * 1024, "conv_tc: TF32 budget");
 
 // wgmma shared-memory matrix descriptor: K-major, SWIZZLE_128B canonical layout (8-row x 128 B atoms, 1024 B apart)
 __device__ __forceinline__ uint64_t make_smem_desc(uint32_t smem_addr) {
@@ -186,7 +205,7 @@ __device__ __forceinline__ void fused_a_row(uint8_t* tile, int r, const TcParams
 // Register budgets (setmaxnreg) of the two roles; 128 producer + 256 consumer threads share the 384 x 168 registers the
 // CTA is launched with.  The FUSED producer runs fused_a_row on all its threads and needs more than the TMA issuer.
 template <bool FUSED> struct TcRegs;
-template <> struct TcRegs<false> { static constexpr int PRODUCER = 40, CONSUMER = 232; };
+template <> struct TcRegs<false> { static constexpr int PRODUCER = 48, CONSUMER = 224; };
 template <> struct TcRegs<true> { static constexpr int PRODUCER = 56, CONSUMER = 224; };
 
 template <int BLOCK_N, int NUM_STAGES, bool FUSED, typename T>
@@ -194,7 +213,7 @@ __global__ void __launch_bounds__(NUM_THREADS, 1)
 conv_tc_kernel(const __grid_constant__ CUtensorMap map_a0, const __grid_constant__ CUtensorMap map_a1,
                const __grid_constant__ CUtensorMap map_a2, const __grid_constant__ CUtensorMap map_b,
                const __grid_constant__ CUtensorMap map_d, const __grid_constant__ CUtensorMap map_r,
-               const TcParams P) {
+               const __grid_constant__ CUtensorMap map_s, const TcParams P) {
   using L = SmemLayout<BLOCK_N, NUM_STAGES, sizeof(T)>;
   using R = TcRegs<FUSED>;
   constexpr bool TF32 = sizeof(T) == 4;
@@ -205,26 +224,31 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap map_a0, const __grid_constant
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023);
 
   uint64_t* bars = reinterpret_cast<uint64_t*>(smem + L::OFF_BARS);
-  uint64_t* full_bar = bars;
-  uint64_t* empty_bar = bars + NUM_STAGES;
+  uint64_t* b_full = bars;
+  uint64_t* b_empty = bars + NUM_STAGES;
+  uint64_t* a_full = bars + 2 * NUM_STAGES;
+  uint64_t* a_empty = a_full + L::A_STAGES;
+  uint64_t* res_bars = a_empty + L::A_STAGES;
 
   const int warp = __shfl_sync(0xffffffffu, threadIdx.x >> 5, 0);   // provably warp-uniform: ptxas sizes each setmaxnreg region
   const int lane = threadIdx.x & 31;
   pdl_trigger();
 
-  // full: the TMA transaction arrival (+ the 128 producer threads' arrivals when FUSED); empty: one arrival per warp
-  // of the consumer warpgroup that read the stage
-  constexpr uint32_t FULL_COUNT = FUSED ? 1 + 128 : 1;
+  // full: the TMA transaction arrival (+ the 128 producer threads' arrivals for A when FUSED); empty: one arrival per
+  // warp of the consumer warpgroup that read the slot
+  constexpr uint32_t A_FULL_COUNT = FUSED ? 1 + 128 : 1;
   if (threadIdx.x == 0) {
     tma_prefetch_desc(&map_a0);
     tma_prefetch_desc(&map_b);
     tma_prefetch_desc(&map_d);
+    if (P.strip_chunks) tma_prefetch_desc(&map_s);
     if (P.nseg > 1) tma_prefetch_desc(&map_a1);
     if (P.nseg > 2) tma_prefetch_desc(&map_a2);
     if (P.has_residual) tma_prefetch_desc(&map_r);
-    for (int i = 0; i < NUM_STAGES; ++i) { mbar_init(&full_bar[i], FULL_COUNT); mbar_init(&empty_bar[i], 4); }
-    mbar_init(bars + 2 * NUM_STAGES, 1);
-    mbar_init(bars + 2 * NUM_STAGES + 1, 1);
+    for (int i = 0; i < NUM_STAGES; ++i) { mbar_init(&b_full[i], 1); mbar_init(&b_empty[i], 4); }
+    for (int i = 0; i < L::A_STAGES; ++i) { mbar_init(&a_full[i], A_FULL_COUNT); mbar_init(&a_empty[i], 4); }
+    mbar_init(res_bars, 1);
+    mbar_init(res_bars + 1, 1);
     mbar_fence_init();
   }
   __syncthreads();
@@ -235,34 +259,58 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap map_a0, const __grid_constant
     setmaxnreg_dec<R::PRODUCER>();
     const int pt = threadIdx.x;                 // 0..127
     if (!FUSED && pt != 0) return;
+    // segment 0's strip chunks (0: per-tap boxes; the fused producer builds per-tap tiles) and the A fills of a tile
+    const int sc = FUSED ? 0 : P.strip_chunks;
+    const int a_fills = tc_a_fills(P.num_k_blocks, sc);
     const int n_local = tc_local_tiles(blockIdx.x, gridDim.x, P.num_tiles);
     for (int j = 0; j < n_local; ++j) {
       const int tile = blockIdx.x + j * gridDim.x;
       const int m_tile = tile % P.num_m_tiles, n_tile = tile / P.num_m_tiles;
       const int tx = m_tile % P.tiles_w, ty = (m_tile / P.tiles_w) % P.tiles_h, tn = m_tile / (P.tiles_w * P.tiles_h);
       const int x0 = tx * P.bw, y0 = ty * P.bh, n0 = tn * P.bn;
-      int kb = 0;
-      for (int s = 0; s < P.nseg; ++s) {
+      // B tile of k-block kb (issue order): packed k-block `col` of the weights
+      auto fill_b = [&](int kb, int col) {
+        const TcSlot sl = tc_slot(j, kb, P.num_k_blocks, NUM_STAGES);
+        mbar_wait(&b_empty[sl.stage], sl.phase ^ 1, P.dbg, 100 + sl.stage);
+        mbar_arrive_expect_tx(&b_full[sl.stage], L::B_TILE_BYTES);
+        tma_load_2d(smem + sl.stage * L::B_TILE_BYTES, &map_b, &b_full[sl.stage], col * BK, n_tile * BLOCK_N);
+      };
+      // segment 0 from strips: fill f = (dx + 1) * sc + chunk, one bw x (bh + 2) box that serves k-blocks 3 f + dy + 1
+      for (int dx = -1; dx <= 1; ++dx)
+        for (int ch = 0; ch < sc; ++ch) {
+          const int f = (dx + 1) * sc + ch;
+          const TcSlot sl = tc_slot(j, f, a_fills, L::A_STAGES);
+          mbar_wait(&a_empty[sl.stage], sl.phase ^ 1, P.dbg, 150 + sl.stage);
+          mbar_arrive_expect_tx(&a_full[sl.stage], P.strip_rows * ROW_BYTES);
+          tma_load_4d(smem + L::OFF_A + sl.stage * L::A_SLOT_BYTES, &map_s, &a_full[sl.stage], ch * BK, x0 + dx, y0 - 1, n0);
+          for (int dy = -1; dy <= 1; ++dy) fill_b(3 * f + dy + 1, tc_strip_column(dx, dy, ch, sc));
+        }
+      // the other k-blocks in packed order, one A box each: k-block kb is column kb and A fill kb - 6 sc
+      int kb = 9 * sc;
+      for (int s = sc ? 1 : 0; s < P.nseg; ++s) {
         const CUtensorMap* ma = s == 0 ? &map_a0 : (s == 1 ? &map_a1 : &map_a2);
         const int taps = P.seg_taps[s];
         for (int tap = 0; tap < taps; ++tap) {
           const int dy = taps == 9 ? tap / 3 - 1 : 0, dx = taps == 9 ? tap % 3 - 1 : 0;
           for (int ch = 0; ch < P.seg_chunks[s]; ++ch, ++kb) {
-            const TcSlot sl = tc_slot(j, kb, P.num_k_blocks, NUM_STAGES);
-            mbar_wait(&empty_bar[sl.stage], sl.phase ^ 1, P.dbg, 100 + sl.stage);
-            uint8_t* sa = smem + sl.stage * L::STAGE_BYTES;
+            const TcSlot sl = tc_slot(j, kb - 6 * sc, a_fills, L::A_STAGES);
+            mbar_wait(&a_empty[sl.stage], sl.phase ^ 1, P.dbg, 150 + sl.stage);
+            uint8_t* sa = smem + L::OFF_A + sl.stage * L::A_SLOT_BYTES;
             const bool build_a = FUSED && s == 0;
             if (pt == 0) {
-              mbar_arrive_expect_tx(&full_bar[sl.stage], build_a ? L::B_TILE_BYTES : L::STAGE_BYTES);
-              if (!build_a) tma_load_4d(sa, ma, &full_bar[sl.stage], ch * BK, x0 + dx, y0 + dy, n0);
-              tma_load_2d(sa + A_TILE_BYTES, &map_b, &full_bar[sl.stage], kb * BK, n_tile * BLOCK_N);
+              if (build_a) mbar_arrive(&a_full[sl.stage]);
+              else {
+                mbar_arrive_expect_tx(&a_full[sl.stage], A_TILE_BYTES);
+                tma_load_4d(sa, ma, &a_full[sl.stage], ch * BK, x0 + dx, y0 + dy, n0);
+              }
+              fill_b(kb, kb);
             }
             if (FUSED) {
               if (build_a) {
                 fused_a_row(sa, pt, P, x0, y0, n0, dx, dy, ch);
                 fence_proxy_async_smem();          // generic-proxy smem writes -> visible to wgmma (async proxy)
               }
-              mbar_arrive(&full_bar[sl.stage]);
+              mbar_arrive(&a_full[sl.stage]);
             }
           }
         }
@@ -273,12 +321,15 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap map_a0, const __grid_constant
 
   // =========================== MMA + epilogue (warpgroups 1, 2) ===========================
   setmaxnreg_inc<R::CONSUMER>();
+  // segment 0's strip chunks (0: per-tap boxes; the fused producer builds per-tap tiles) and the A fills of a tile
+  const int sc = FUSED ? 0 : P.strip_chunks;
+  const int a_fills = tc_a_fills(P.num_k_blocks, sc);
   const int wg = warp / 4 - 1;                 // consumer warpgroup: takes the local tiles j with tc_consumer_of(j) == wg
   const int wt = threadIdx.x & 127;
   const int rps = P.bw * P.bh;                 // rows per sample inside a tile
   uint8_t* staging = smem + L::OFF_STAGING + wg * L::STAGING_BYTES;
   float* stats_sm = reinterpret_cast<float*>(smem + L::OFF_STATS + wg * L::STATS_BYTES);
-  uint64_t* res_full = bars + 2 * NUM_STAGES + wg;
+  uint64_t* res_full = res_bars + wg;
   // named barriers: 1 + wg = this warpgroup's epilogue (128 threads); 3 + wg = "warpgroup wg may issue its MMAs", which
   // the other warpgroup arrives on once its own mainloop has issued (256 threads: 128 arrive, 128 sync)
   const int epi_bar = 1 + wg, my_turn = 3 + wg, other_turn = 4 - wg;
@@ -304,15 +355,18 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap map_a0, const __grid_constant
         tma_load_4d(staging + c * A_TILE_BYTES, &map_r, res_full, c_tile + c * BK, x0, y0, n0);
     }
 
-    // the other warpgroup has waited for every stage of the tile before this one: the ring's parities are unambiguous
+    // the other warpgroup has waited for every slot of the tile before this one: both rings' parities are unambiguous
     if (j > 0) named_bar_sync(my_turn, 256);
-    int prev = -1;
+    int prev_b = -1, prev_a = -1;              // slots to release once the previous k-block retires (-1: A still in use)
     for (int kb = 0; kb < P.num_k_blocks; ++kb) {
-      const TcSlot sl = tc_slot(j, kb, P.num_k_blocks, NUM_STAGES);
-      mbar_wait(&full_bar[sl.stage], sl.phase, P.dbg, 300 + 10 * wg + sl.stage);
-      const uint32_t a_addr = smem_u32(smem + sl.stage * L::STAGE_BYTES);
-      const uint64_t adesc = make_smem_desc(a_addr);
-      const uint64_t bdesc = make_smem_desc(a_addr + A_TILE_BYTES);
+      const TcSlot sb = tc_slot(j, kb, P.num_k_blocks, NUM_STAGES);
+      const TcAUse u = tc_a_use(kb, sc);
+      const TcSlot sa = tc_slot(j, u.fill, a_fills, L::A_STAGES);
+      mbar_wait(&a_full[sa.stage], sa.phase, P.dbg, 350 + 10 * wg + sa.stage);
+      mbar_wait(&b_full[sb.stage], sb.phase, P.dbg, 300 + 10 * wg + sb.stage);
+      // a strip tap's tile starts (dy + 1) * bw rows (whole 1024 B swizzle atoms) into the strip
+      const uint64_t adesc = make_smem_desc(smem_u32(smem + L::OFF_A + sa.stage * L::A_SLOT_BYTES) + u.dy1 * P.bw * ROW_BYTES);
+      const uint64_t bdesc = make_smem_desc(smem_u32(smem + sb.stage * L::B_TILE_BYTES));
       wgmma_fence();
 #pragma unroll
       for (int k = 0; k < BK / WK; ++k) {
@@ -322,14 +376,24 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap map_a0, const __grid_constant
         wgmma_tile<BLOCK_N, T>(acc[1], adesc + (uint64_t)(512 + 2 * k), bdesc + (uint64_t)(2 * k), (kb | k) != 0);
       }
       wgmma_commit();
-      wgmma_wait<1>();                         // the previous k-block's MMAs have retired: its stage is free
-      if (prev >= 0) { __syncwarp(); if (lane == 0) mbar_arrive(&empty_bar[prev]); }
-      prev = sl.stage;
+      wgmma_wait<1>();                         // the previous k-block's MMAs have retired: its B stage is free, and its
+      if (prev_b >= 0) {                       // A slot too if it was that fill's last reader
+        __syncwarp();
+        if (lane == 0) {
+          mbar_arrive(&b_empty[prev_b]);
+          if (prev_a >= 0) mbar_arrive(&a_empty[prev_a]);
+        }
+      }
+      prev_b = sb.stage;
+      prev_a = u.last ? sa.stage : -1;
     }
     if (j + 1 < n_local) named_bar_arrive(other_turn, 256);
     wgmma_wait<0>();
     __syncwarp();
-    if (lane == 0) mbar_arrive(&empty_bar[prev]);
+    if (lane == 0) {                           // a tile's last k-block is always the last reader of its A fill
+      mbar_arrive(&b_empty[prev_b]);
+      mbar_arrive(&a_empty[prev_a]);
+    }
 
     if (P.has_residual) {
       mbar_wait(res_full, res_phase, P.dbg, 400 + wg);
@@ -568,6 +632,11 @@ void launch_impl(cudaStream_t st, const ConvArgs& a, TensorDesc& out, int* dbg, 
     }
   }
   P.num_k_blocks = kblocks;
+  // segment 0 from dy-halo strips where the box allows it (the fused producer builds per-tap tiles itself)
+  P.strip_rows = FUSED ? 0 : tc_strip_rows(bw, bh, bn, a.seg[0].taps);
+  P.strip_chunks = P.strip_rows ? P.seg_chunks[0] : 0;
+  const TensorDesc& s0 = a.seg[0].src;
+  const CUtensorMap ms = P.strip_rows ? make_act_map(s0.p, s0.N, s0.H, s0.W, s0.C, bw, bh + 2, 1, ES) : ma[0];
   if (FUSED) {
     P.raw0 = static_cast<const __half*>(a.seg[0].src.p); P.c0 = a.seg[0].src.C;
     P.raw1 = a.gn_has_cat ? static_cast<const __half*>(a.gn_cat.p) : nullptr; P.c1 = a.gn_has_cat ? a.gn_cat.C : 0;
@@ -588,7 +657,7 @@ void launch_impl(cudaStream_t st, const ConvArgs& a, TensorDesc& out, int* dbg, 
   if (first_use_on_device(attr_devs)) {
     CUDA_OK(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, L::DYN_BYTES));
   }
-  launch_k(kern, dim3(plan.grid), dim3(NUM_THREADS), (size_t)L::DYN_BYTES, st, ma[0], ma[1], ma[2], mb, md, mr, P);
+  launch_k(kern, dim3(plan.grid), dim3(NUM_THREADS), (size_t)L::DYN_BYTES, st, ma[0], ma[1], ma[2], mb, md, mr, ms, P);
   CUDA_OK(cudaGetLastError());
 }
 
