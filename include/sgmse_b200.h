@@ -216,14 +216,23 @@ int sgmse_b200_enhance_ode(sgmse_b200_engine* e, const float* wav, int B, int L,
                            const void* prior_noise, float* out, int host_buffers, int* nfe, void* stream);
 
 /* Introspection / debugging */
-/* bytes of activation workspace one forward pass of (B, F, T) needs; host-only (no CUDA call); -1 on error */
+/* bytes of all activation buffers of one forward pass of (B, F, T), each in a range of its own (the layout without
+ * reuse); host-only (no CUDA call); -1 on error.  The engine allocates the planned size, see sgmse_b200_workspace_plan. */
 long long sgmse_b200_workspace_bytes(sgmse_b200_engine* e, int B, int F, int T);
+/* The workspace plan of one forward pass of (B, F, T) with the engine's current options ("record_taps" included):
+ * returns the bytes of activation workspace the engine allocates for it, -1 on error.  Host-only (no CUDA call).
+ * Each buffer of the forward, in allocation order, is live from step `first` to step `last` (step s: the s-th launch of
+ * the forward; last == *n_steps: read after the forward returns).  Buffers whose lifetimes intersect never overlap.
+ * rows (nullable): [cap][5] of (offset, bytes, first, last, tapped); n_bufs, n_steps nullable. */
+long long sgmse_b200_workspace_plan(sgmse_b200_engine* e, int B, int F, int T, long long* rows, long long cap,
+                                    long long* n_bufs, int* n_steps);
 /* copy a recorded intermediate activation (see sgmse_b200_set_option "record_taps") as fp32 NCHW to host */
 int sgmse_b200_get_tap(sgmse_b200_engine* e, const char* name, float* out_host, long long cap, int shape[4]);
 /* options: "record_taps" (0/1), "use_graphs" (0/1), "tc_mask" (bit i set = conv class i may use the wgmma kernel),
  * "time_convs" (0/1: bracket every convolution launch with CUDA events; disables graph replay),
  * "lanes" (1..8 concurrent launch sequences inside a captured sampler graph), "max_graphs" (captured sampler graphs kept,
- * least recently used evicted; default 16).  The kernel A/B switches the tools use ("tc_variant", "attn_variant",
+ * least recently used evicted; default 16), "workspace_poison" (0/1, for tests: fill each workspace buffer with 0xFF
+ * bytes, NaN in fp16 and fp32, right after its last reader is enqueued).  The kernel A/B switches the tools use ("tc_variant", "attn_variant",
  * "fir_variant", "inconv_variant", "outconv_variant", "combine_variant", "tc1_narrow", "gn_self", "gnfin_variant") are
  * state of THIS engine: every entry point installs the calling engine's selection before it launches anything, so another
  * engine of the same process (another device, another host thread) never sees them, and a captured sampler graph keeps

@@ -76,6 +76,8 @@ SYMBOLS = {
     "sgmse_b200_enhance_ode": (C.c_int, [_P, _P, C.c_int, C.c_int, C.POINTER(Ode), C.c_int, _P, _P, C.c_int, _P, _P]),
     "sgmse_b200_get_tap": (C.c_int, [_P, C.c_char_p, _P, C.c_longlong, C.POINTER(C.c_int * 4)]),
     "sgmse_b200_workspace_bytes": (C.c_longlong, [_P, C.c_int, C.c_int, C.c_int]),
+    "sgmse_b200_workspace_plan": (C.c_longlong, [_P, C.c_int, C.c_int, C.c_int, _P, C.c_longlong,
+                                                 C.POINTER(C.c_longlong), C.POINTER(C.c_int)]),
     "sgmse_b200_set_option": (C.c_int, [_P, C.c_char_p, C.c_longlong]),
     "sgmse_b200_get_counter": (C.c_longlong, [_P, C.c_char_p]),
 }

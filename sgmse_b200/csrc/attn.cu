@@ -141,6 +141,136 @@ static void run(cudaStream_t st, const TensorDesc& qkv, TensorDesc& out, int S, 
   kern<<<grid, 128, smem, st>>>((const T*)qkv.p, S, C, 1.0f / sqrtf((float)C), (T*)out.p);
   CUDA_OK(cudaGetLastError());
 }
+
+// fp32 storage at any token count: the full score row of attention_kernel outgrows shared memory past S ~ 4 700
+// (C = 256).  Flash-style instead: a block keeps 32 queries resident, streams keys and values through shared memory in
+// tiles of KT and keeps a running max and sum per query (online softmax).  fp32 CUDA-core FMAs throughout, as every
+// non-convolution kernel of the fp32 and tf32_tc modes.  Thread (tq, tk): queries 4 tq .. 4 tq + 3; keys tk + 16 j of a
+// tile for the scores, channels tk + 16 j of the output.
+constexpr int SQT = 32;
+template <int C>
+size_t stream_smem() { return ((size_t)(SQT + KT) * (C + 1) + SQT * (KT + 1) + 2 * SQT) * sizeof(float); }
+
+template <int C>
+__global__ void __launch_bounds__(128) attention_stream_kernel(const float* __restrict__ qkv, int S, float scale_log2e,
+                                                               float* __restrict__ out) {
+  constexpr int LD = C + 1, LDP = KT + 1, CPT = C / 16;
+  extern __shared__ float sm[];
+  float* Qs = sm;                    // [SQT][LD]
+  float* KVs = Qs + SQT * LD;        // [KT][LD]: the key tile, then the value tile
+  float* Ps = KVs + KT * LD;         // [SQT][LDP]: scores, then probabilities (log2 domain)
+  float* alpha = Ps + SQT * LDP;     // [SQT]: rescale factor of the running output for this tile
+  float* lsum = alpha + SQT;         // [SQT]: final softmax denominators
+  const int n = blockIdx.y, q0 = blockIdx.x * SQT;
+  const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
+  const int tq = tid / 16, tk = tid % 16;
+  const float* base = qkv + (size_t)n * S * 3 * C;
+
+  auto load_tile = [&](float* dst, int rows, int row0, int col0) {
+    for (int i = tid; i < rows * (C / 4); i += 128) {
+      const int r = i / (C / 4), cv = i % (C / 4);
+      float4 v = make_float4(0.f, 0.f, 0.f, 0.f);
+      if (row0 + r < S) v = *reinterpret_cast<const float4*>(base + (size_t)(row0 + r) * 3 * C + col0 + cv * 4);
+      float* d = dst + r * LD + cv * 4;
+      d[0] = v.x; d[1] = v.y; d[2] = v.z; d[3] = v.w;
+    }
+  };
+  load_tile(Qs, SQT, q0, 0);
+
+  float o[4][CPT];
+#pragma unroll
+  for (int i = 0; i < 4; ++i)
+#pragma unroll
+    for (int j = 0; j < CPT; ++j) o[i][j] = 0.f;
+  float mrow[SQT / 4], lrow[SQT / 4];          // rows warp * 8 + r, replicated over the warp's lanes
+#pragma unroll
+  for (int r = 0; r < SQT / 4; ++r) { mrow[r] = -INFINITY; lrow[r] = 0.f; }
+
+  for (int k0 = 0; k0 < S; k0 += KT) {
+    __syncthreads();                           // previous tile's P V done with KVs and Ps
+    load_tile(KVs, KT, k0, C);
+    __syncthreads();
+    float acc[4][4];
+#pragma unroll
+    for (int i = 0; i < 4; ++i)
+#pragma unroll
+      for (int j = 0; j < 4; ++j) acc[i][j] = 0.f;
+    for (int c = 0; c < C; ++c) {
+      float qv[4], kv[4];
+#pragma unroll
+      for (int i = 0; i < 4; ++i) qv[i] = Qs[(tq * 4 + i) * LD + c];
+#pragma unroll
+      for (int j = 0; j < 4; ++j) kv[j] = KVs[(tk + 16 * j) * LD + c];
+#pragma unroll
+      for (int i = 0; i < 4; ++i)
+#pragma unroll
+        for (int j = 0; j < 4; ++j) acc[i][j] = fmaf(qv[i], kv[j], acc[i][j]);
+    }
+#pragma unroll
+    for (int i = 0; i < 4; ++i)
+#pragma unroll
+      for (int j = 0; j < 4; ++j)
+        Ps[(tq * 4 + i) * LDP + tk + 16 * j] = k0 + tk + 16 * j < S ? acc[i][j] * scale_log2e : -INFINITY;
+    __syncthreads();                           // scores complete; the key tile is no longer read
+    // online softmax: warp w owns rows 8 w .. 8 w + 7, two keys per lane
+#pragma unroll
+    for (int r = 0; r < SQT / 4; ++r) {
+      float* row = Ps + (warp * (SQT / 4) + r) * LDP;
+      const float s0 = row[lane], s1 = row[lane + 32];
+      float mx = fmaxf(s0, s1);
+      for (int of = 16; of > 0; of >>= 1) mx = fmaxf(mx, __shfl_xor_sync(0xffffffffu, mx, of));
+      mx = fmaxf(mx, mrow[r]);                 // finite: key k0 of the first tile is always a real token
+      const float p0 = exp2f(s0 - mx), p1 = exp2f(s1 - mx);
+      row[lane] = p0; row[lane + 32] = p1;
+      float sum = p0 + p1;
+      for (int of = 16; of > 0; of >>= 1) sum += __shfl_xor_sync(0xffffffffu, sum, of);
+      const float a = exp2f(mrow[r] - mx);
+      lrow[r] = lrow[r] * a + sum;
+      mrow[r] = mx;
+      if (lane == 0) alpha[warp * (SQT / 4) + r] = a;
+    }
+    load_tile(KVs, KT, k0, 2 * C);             // value tile (zero past S, where p = 0 as well)
+    __syncthreads();
+#pragma unroll
+    for (int i = 0; i < 4; ++i) {
+      const float a = alpha[tq * 4 + i];
+#pragma unroll
+      for (int j = 0; j < CPT; ++j) o[i][j] *= a;
+    }
+    for (int k = 0; k < KT; ++k) {
+      float p[4];
+#pragma unroll
+      for (int i = 0; i < 4; ++i) p[i] = Ps[(tq * 4 + i) * LDP + k];
+#pragma unroll
+      for (int j = 0; j < CPT; ++j) {
+        const float v = KVs[k * LD + tk + 16 * j];
+#pragma unroll
+        for (int i = 0; i < 4; ++i) o[i][j] = fmaf(p[i], v, o[i][j]);
+      }
+    }
+  }
+  if (lane == 0)
+#pragma unroll
+    for (int r = 0; r < SQT / 4; ++r) lsum[warp * (SQT / 4) + r] = lrow[r];
+  __syncthreads();
+#pragma unroll
+  for (int i = 0; i < 4; ++i) {
+    const int q = q0 + tq * 4 + i;
+    if (q >= S) continue;
+    const float inv = 1.f / lsum[tq * 4 + i];
+#pragma unroll
+    for (int j = 0; j < CPT; ++j) out[((size_t)n * S + q) * C + tk + 16 * j] = o[i][j] * inv;
+  }
+}
+
+template <int C>
+void run_stream(cudaStream_t st, const TensorDesc& qkv, TensorDesc& out, int S) {
+  auto kern = attention_stream_kernel<C>;
+  CUDA_OK(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)stream_smem<C>()));
+  dim3 grid(cdiv(S, SQT), qkv.N);
+  kern<<<grid, 128, stream_smem<C>(), st>>>((const float*)qkv.p, S, 1.4426950408889634f / sqrtf((float)C), (float*)out.p);
+  CUDA_OK(cudaGetLastError());
+}
 }  // namespace
 
 // ------------------------------------------------------------------------------------------------
@@ -315,6 +445,10 @@ void launch_attention(cudaStream_t st, const TensorDesc& qkv, TensorDesc& out) {
   int QT = 32;
   if (smem_for(32) > lim) QT = 16;
   if (QT == 16 && smem_for(16) > lim) QT = 8;
+  if (smem_for(QT) > lim && qkv.dt == DT_F32) {  // the full score row does not fit: stream the keys
+    if (C == 256) { run_stream<256>(st, qkv, out, S); return; }
+    if (C == 128) { run_stream<128>(st, qkv, out, S); return; }
+  }
   SG_CHECK(smem_for(QT) <= lim, "attention: %d tokens x %d channels does not fit the v1 kernel", S, C);
 #define GO(T) \
   do { if (QT == 32) run<T, 32>(st, qkv, out, S, C, smem_for(32)); \

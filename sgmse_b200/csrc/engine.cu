@@ -1,5 +1,5 @@
 // Host side of the engine: architecture walk, weight packing, the network forward pass as a static
-// launch sequence over a bump-allocated workspace, the predictor-corrector loop (captured as one CUDA
+// launch sequence over a liveness-planned workspace, the predictor-corrector loop (captured as one CUDA
 // graph), the cuFFT STFT/iSTFT front/back end, and the C-ABI of include/sgmse_b200.h.
 //
 // Reference call stack replaced: ScoreModel.enhance (model.py:426-465) -> get_pc_sampler
@@ -487,6 +487,8 @@ TembWeights temb_weights(const Engine& e) {
 // ------------------------------------------------------------------------------------------------
 // forward pass
 // ------------------------------------------------------------------------------------------------
+const WsPlan& ensure_arena(Engine& e, int B, int F, int T);
+
 struct Fwd {
   Engine& e;
   cudaStream_t st;
@@ -499,19 +501,50 @@ struct Fwd {
   TensorDesc act(int N, int H, int W, int C, bool stats) {
     TensorDesc t;
     t.N = N; t.H = H; t.W = W; t.C = C; t.dt = dt;
+    // element offsets are 64-bit, but several kernels index pixels x channels of one tensor in 32 bits
+    SG_CHECK(t.numel() < ((size_t)1 << 31), "a [%d, %d, %d, %d] activation has 2^31 elements or more: the batch or clip is "
+             "too long for one forward (16 kHz: T < 32768 frames per utterance, 48 kHz: T < 10923)", N, C, H, W);
     t.p = e.arena.alloc(t.bytes());
     if (stats) t.stats = (float*)e.arena.alloc(t.stats_capacity_floats() * 4);
     return t;
   }
   float4* act4(int N, int H, int W) { return (float4*)e.arena.alloc((size_t)N * H * W * 16); }
-  void count(int n = 1) { e.kernel_launches += n; e.launches_this_forward += n; }
-  void tap(const std::string& name, const TensorDesc& t) { if (e.record_taps && !dry) e.taps[name] = t; }
+  void tap(const std::string& name, const TensorDesc& t) {
+    if (!e.record_taps) return;
+    if (dry) { e.arena.keep(t.p, true); e.arena.keep(t.stats, true); }
+    else e.taps[name] = t;
+  }
   void tap4(const std::string& name, const float4* p, int N, int H, int W) {
-    if (e.record_taps && !dry) e.taps4[name] = {p, {N, 4, H, W}};
+    if (!e.record_taps) return;
+    if (dry) e.arena.keep(p, true);
+    else e.taps4[name] = {p, {N, 4, H, W}};
+  }
+
+  // Lifetimes (planning run): every launch site ends with step(...) naming each arena buffer the launch reads or
+  // writes, so a buffer's last step is the launch of its last reader.  Run mode: counts the launch and, with
+  // workspace_poison, fills the buffers that launch was the last reader of.
+  void mark(const void* p) { e.arena.use(p); }
+  void mark(const TensorDesc& t) { mark(t.p); mark(t.stats); }
+  void mark(const TensorDesc* t) { if (t) mark(*t); }
+  void mark(const ConvArgs& a) {
+    for (int i = 0; i < a.nseg; ++i) mark(a.seg[i].src);
+    mark(a.residual);
+    mark((const void*)a.gn_ab);
+    if (a.gn_has_cat) mark(a.gn_cat);
+  }
+  template <typename... A> void step(const A&... bufs) {
+    if (dry) { (mark(bufs), ...); ++e.arena.step; return; }
+    e.kernel_launches += 1; e.launches_this_forward += 1;
+    if (e.workspace_poison)
+      for (int b : e.arena.plan->ends[e.arena.step]) {
+        const WsBuf& w = e.arena.plan->bufs[b];
+        CUDA_OK(cudaMemsetAsync(e.arena.base + w.off, 0xFF, w.bytes, st));
+      }
+    ++e.arena.step;
   }
 
   void conv(const ConvArgs& a, TensorDesc& out, int cls) {
-    if (dry) return;
+    if (dry) { step(a, out); return; }
     const bool want_tc = tc_mode(e.cfg) && ((e.tc_mask >> cls) & 1);
     const bool tc = a.gn_ab != nullptr || (want_tc && conv_tc_supported(a, out));
     cudaEvent_t ev0 = nullptr, ev1 = nullptr;
@@ -528,7 +561,7 @@ struct Fwd {
                            [&] { double b = 0; for (int i = 0; i < a.nseg; ++i) b += (double)a.seg[i].src.bytes(); return b; }();
       e.conv_events.push_back(ConvTiming{ev0, ev1, flops, bytes, tc});
     }
-    count();
+    step(a, out);
   }
 
   // `plain_consumer`: the only reader of (a, b) is apply_plain below -- with the gn_self candidate it rebuilds the
@@ -539,18 +572,20 @@ struct Fwd {
     float2* ab = (float2*)e.arena.alloc((size_t)x0.N * Ct * sizeof(float2));
     const int groups = gn_groups(Ct);
     if (plain_consumer && gn_self_applies(x0, x1)) return ab;
-    if (!dry) { launch_gn_finalize(st, x0, x1, e.blob_dev + g_off, e.blob_dev + b_off, groups, ab, e.range_flag); count(); }
+    if (!dry) launch_gn_finalize(st, x0, x1, e.blob_dev + g_off, e.blob_dev + b_off, groups, ab, e.range_flag);
+    step(x0, x1, ab);
     return ab;
   }
   // y = [silu](a x + b) without resampling: gn_apply_plain on the finalized table, or (gn_self) finalize + apply in one kernel
   void apply_plain(const TensorDesc& x0, const TensorDesc* x1, const float2* ab, long long g_off, long long b_off, bool silu,
                    TensorDesc& out) {
-    if (dry) return;
-    if (gn_self_applies(x0, x1))
-      launch_gn_norm_apply(st, x0, x1, e.blob_dev + g_off, e.blob_dev + b_off, gn_groups(x0.C + (x1 ? x1->C : 0)), silu, out, e.range_flag);
-    else
-      launch_gn_apply(st, x0, x1, ab, silu, RS_NONE, out, nullptr);
-    count();
+    if (!dry) {
+      if (gn_self_applies(x0, x1))
+        launch_gn_norm_apply(st, x0, x1, e.blob_dev + g_off, e.blob_dev + b_off, gn_groups(x0.C + (x1 ? x1->C : 0)), silu, out, e.range_flag);
+      else
+        launch_gn_apply(st, x0, x1, ab, silu, RS_NONE, out, nullptr);
+    }
+    step(x0, x1, ab, out);
   }
 
   TensorDesc resblock(const Layer& l, const TensorDesc& x0, const TensorDesc* x1) {
@@ -572,7 +607,8 @@ struct Fwd {
       SG_CHECK(!x1, "resampling resblock with concatenated input");
       h0 = act(N, Ho, Wo, Ct, false);
       xr = act(N, Ho, Wo, Ct, false);
-      if (!dry) { launch_gn_apply(st, x0, nullptr, ab0, true, rs, h0, &xr); count(); }
+      if (!dry) launch_gn_apply(st, x0, nullptr, ab0, true, rs, h0, &xr);
+      step(x0, ab0, h0, xr);
     } else if (!fuse0) {
       h0 = act(N, Ho, Wo, Ct, false);
       apply_plain(x0, x1, ab0, l.gn0_w, l.gn0_b, true, h0);
@@ -635,7 +671,8 @@ struct Fwd {
       conv(a, qkv, 2);
     }
     TensorDesc av = act(x.N, x.H, x.W, C, false);
-    if (!dry) { launch_attention(st, qkv, av); count(); }
+    if (!dry) launch_attention(st, qkv, av);
+    step(qkv, av);
     TensorDesc out = act(x.N, x.H, x.W, C, true);
     {
       ConvArgs a;
@@ -653,13 +690,15 @@ struct Fwd {
     float2* ab = gn(h, nullptr, l.gn0_w, l.gn0_b, !out_conv_fuses_gn(h));
     if (out_conv_fuses_gn(h)) {                    // GroupNorm-apply + SiLU happen while the conv stages its tile
       float4* out = act4(h.N, h.H, h.W);
-      if (!dry) { launch_out_conv(st, h, l.small_w, l.out_bias_host, addend, out, ab, l.small_wfrag); count(); }
+      if (!dry) launch_out_conv(st, h, l.small_w, l.out_bias_host, addend, out, ab, l.small_wfrag);
+      step(h, ab, addend, out);
       return out;
     }
     TensorDesc a = act(h.N, h.H, h.W, h.C, false);
     apply_plain(h, nullptr, ab, l.gn0_w, l.gn0_b, true, a);
     float4* out = act4(h.N, h.H, h.W);
-    if (!dry) { launch_out_conv(st, a, l.small_w, l.out_bias_host, addend, out, nullptr, l.small_wfrag); count(); }
+    if (!dry) launch_out_conv(st, a, l.small_w, l.out_bias_host, addend, out, nullptr, l.small_wfrag);
+    step(a, addend, out);
     return out;
   }
 
@@ -670,7 +709,8 @@ struct Fwd {
     SG_CHECK(H % (1 << (L - 1)) == 0 && W % (1 << (L - 1)) == 0, "F=%d, T=%d must be multiples of %d", H, W, 1 << (L - 1));
     if (c.num_attn_resolutions > 0 && c.backbone != SGMSE_B200_BACKBONE_NCSNPP_48K)
       SG_CHECK(H == c.image_size, "ncsnpp places attention for F == image_size == %d (got F=%d), see ncsnpp.py:84,308", c.image_size, H);
-    e.arena.reset();
+    if (dry) e.arena.begin(nullptr);
+    else e.arena.begin(&ensure_arena(e, B, H, W));
     e.launches_this_forward = 0;
     e.tc_convs = e.direct_convs = 0;
     if (e.record_taps && !dry) { e.taps.clear(); e.taps4.clear(); }
@@ -684,7 +724,8 @@ struct Fwd {
     std::vector<TensorDesc> hs;
     {
       TensorDesc h0 = act(B, H, W, c.nf, true);
-      if (!dry) { launch_input_conv(st, state, B, H, W, e.inconv_w_packed, e.blob_dev + e.inconv_b, h0, in_scale); count(); }
+      if (!dry) launch_input_conv(st, state, B, H, W, e.inconv_w_packed, e.blob_dev + e.inconv_b, h0, in_scale);
+      step(h0);
       tap("in_conv", h0);
       hs.push_back(h0);
     }
@@ -702,10 +743,12 @@ struct Fwd {
           const Layer& l = next(LK_COMBINE);
           float4* pd = act4(B, ph / 2, pw / 2);
           // the input pyramid starts at the network input c_in * (x, y) (ncsnpp.py:293-296): the first level carries c_in
-          if (!dry) { launch_fir4(st, pyr_in, B, ph, pw, RS_DOWN, pd, pyr_in == state ? in_scale : 1.f); count(); }
+          if (!dry) launch_fir4(st, pyr_in, B, ph, pw, RS_DOWN, pd, pyr_in == state ? in_scale : 1.f);
+          step(pyr_in, pd);
           pyr_in = pd; ph /= 2; pw /= 2;
           TensorDesc o = act(B, h.H, h.W, h.C, true);
-          if (!dry) { launch_combine(st, pyr_in, l.small_w, l.small_b, h, o); count(); }
+          if (!dry) launch_combine(st, pyr_in, l.small_w, l.small_b, h, o);
+          step(pyr_in, h, o);
           tap("m" + std::to_string(l.idx), o);
           h = o;
         }
@@ -731,7 +774,8 @@ struct Fwd {
         const float4* add = nullptr;
         if (pyramid) {
           float4* up = act4(B, qh * 2, qw * 2);
-          if (!dry) { launch_fir4(st, pyramid, B, qh, qw, RS_UP, up); count(); }
+          if (!dry) launch_fir4(st, pyramid, B, qh, qw, RS_UP, up);
+          step(pyramid, up);
           add = up;
         }
         pyramid = outconv(l, h, add);
@@ -746,9 +790,69 @@ struct Fwd {
       tap4("pyr0", pyramid, B, h.H, h.W);
     }
     SG_CHECK(it == e.layers.size(), "internal: %zu of %zu layers consumed", it, e.layers.size());
+    if (dry) e.arena.keep(pyramid, false);   // read by the output layer / sampler update after the forward
+    else SG_CHECK(e.arena.step == e.arena.plan->steps && e.arena.next == e.arena.plan->bufs.size(),
+                  "internal: the forward departed from its workspace plan");
     return pyramid;
   }
 };
+
+// Interval packing of one forward's buffers (planning run in e.arena.rec).  Largest buffers first (ties: earlier
+// allocation first), each at the lowest 256-B aligned offset that overlaps no placed buffer whose lifetime
+// intersects its own.  Deterministic: the layout depends on the shapes and the launch sequence alone.
+//
+// Reuse is safe because every launch of one forward is enqueued on one stream (each lane has its own arena and
+// stream): a buffer placed over a dead one is first written by a launch that follows, in stream order, the dead
+// buffer's last reader.  With programmatic dependent launch every kernel waits for its predecessor's completion
+// before its first global access (common.cuh), which keeps that order.
+WsPlan pack_workspace(std::vector<WsBuf> bufs, int steps) {
+  WsPlan p;
+  p.steps = steps;
+  p.ends.assign(steps, {});
+  for (WsBuf& b : bufs) {
+    p.bump = ((p.bump + 255) & ~(size_t)255) + b.bytes;
+    if (b.last == INT_MAX) b.last = steps;
+  }
+  std::vector<int> order(bufs.size());
+  for (size_t i = 0; i < order.size(); ++i) order[i] = (int)i;
+  std::stable_sort(order.begin(), order.end(), [&](int a, int b) { return bufs[a].bytes > bufs[b].bytes; });
+  std::vector<int> placed, conflicts;
+  for (int i : order) {
+    WsBuf& b = bufs[i];
+    conflicts.clear();
+    for (int j : placed)
+      if (bufs[j].first <= b.last && b.first <= bufs[j].last) conflicts.push_back(j);
+    std::sort(conflicts.begin(), conflicts.end(), [&](int x, int y) { return bufs[x].off < bufs[y].off; });
+    size_t off = 0;
+    for (int j : conflicts) {
+      if (off + b.bytes <= bufs[j].off) break;
+      off = std::max(off, (bufs[j].off + bufs[j].bytes + 255) & ~(size_t)255);
+    }
+    b.off = off;
+    p.bytes = std::max(p.bytes, off + b.bytes);
+    placed.push_back(i);
+    if (b.last < steps) p.ends[b.last].push_back(i);
+  }
+  p.bytes += 4096;
+  p.bufs = std::move(bufs);
+  return p;
+}
+
+// The workspace layout of one forward of (B, F, T) with the engine's current options: planned once by a host-only
+// run of the launch sequence, then cached.
+const WsPlan& workspace_plan(Engine& e, int B, int F, int T) {
+  const auto key = std::make_tuple(B, F, T, e.record_taps);
+  auto it = e.ws_plans.find(key);
+  if (it != e.ws_plans.end()) return it->second;
+  Arena saved = e.arena;
+  e.arena = Arena{};
+  e.arena.dry = true;
+  Fwd f{e, nullptr, nullptr, 0, true, act_dtype(e.cfg)};
+  try { f.run(nullptr, B, F, T); } catch (...) { e.arena = saved; throw; }
+  WsPlan p = pack_workspace(std::move(e.arena.rec), e.arena.step);
+  e.arena = saved;
+  return e.ws_plans.emplace(key, std::move(p)).first->second;
+}
 
 void clear_graphs(Engine& e) {
   for (auto& g : e.graphs) cudaGraphExecDestroy(g.second.exec);
@@ -802,29 +906,18 @@ void ensure_lanes(Engine& e, int want) {
   }
 }
 
-// Workspace for one forward pass of (B, F, T).  The bump allocation is replayed identically by every
-// forward of the same shape, so buffer addresses (and with them captured graphs) stay valid as long as
-// the arena itself is not re-allocated.
-void ensure_arena(Engine& e, int B, int F, int T) {
-  const auto key = std::make_tuple(B, F, T);
-  auto it = e.arena_need.find(key);
-  if (it == e.arena_need.end()) {
-    Arena saved = e.arena;
-    e.arena = Arena{};
-    e.arena.dry = true;
-    Fwd f{e, nullptr, nullptr, 0, true, act_dtype(e.cfg)};
-    f.run(nullptr, B, F, T);
-    const size_t need = e.arena.high + 4096;
-    e.arena = saved;
-    it = e.arena_need.emplace(key, need).first;
-  }
-  if (it->second > e.arena.cap) {
+// Workspace for one forward pass of (B, F, T).  Every forward of a shape follows the same cached plan, so buffer
+// addresses (and with them captured graphs) stay valid as long as the arena itself is not re-allocated.
+const WsPlan& ensure_arena(Engine& e, int B, int F, int T) {
+  const WsPlan& p = workspace_plan(e, B, F, T);
+  if (p.bytes > e.arena.cap) {
     clear_graphs(e);
     if (e.arena.base) { CUDA_OK(cudaDeviceSynchronize()); cudaFree(e.arena.base); e.arena.base = nullptr; e.arena.cap = 0; }
-    CUDA_OK(cudaMalloc((void**)&e.arena.base, it->second));
-    e.arena.cap = it->second;
+    CUDA_OK(cudaMalloc((void**)&e.arena.base, p.bytes));
+    e.arena.cap = p.bytes;
   }
   e.arena.dry = false;
+  return p;
 }
 
 template <typename T>
@@ -1924,18 +2017,32 @@ int sgmse_b200_get_tap(sgmse_b200_engine* e, const char* name, float* out_host, 
 }
 
 long long sgmse_b200_workspace_bytes(sgmse_b200_engine* e, int B, int F, int T) {
-  // host-only dry run of the launch sequence (no CUDA call): exercises the whole layer walk
+  // host-only planning run of the launch sequence (no CUDA call): exercises the whole layer walk
   try {
     SG_CHECK(e && B > 0, "bad argument");
     activate(*e);
-    Arena saved = e->arena;
-    e->arena = Arena{};
-    e->arena.dry = true;
-    Fwd f{*e, nullptr, nullptr, 0, true, act_dtype(e->cfg)};
-    try { f.run(nullptr, B, F, T); } catch (...) { e->arena = saved; throw; }
-    const long long need = (long long)e->arena.high + 4096;
-    e->arena = saved;
-    return need;
+    return (long long)workspace_plan(*e, B, F, T).bump + 4096;
+  } catch (const sgmse::Error& err) { sgmse::set_last_error(err.msg); return -1; }
+  catch (...) { sgmse::set_last_error("unknown error"); return -1; }
+}
+
+long long sgmse_b200_workspace_plan(sgmse_b200_engine* e, int B, int F, int T, long long* rows, long long cap,
+                                    long long* n_bufs, int* n_steps) {
+  try {
+    SG_CHECK(e && B > 0, "bad argument");
+    activate(*e);
+    const WsPlan& p = workspace_plan(*e, B, F, T);
+    if (n_bufs) *n_bufs = (long long)p.bufs.size();
+    if (n_steps) *n_steps = p.steps;
+    if (rows) {
+      SG_CHECK(cap >= (long long)p.bufs.size(), "plan buffer holds %lld rows, the plan has %zu", cap, p.bufs.size());
+      for (size_t i = 0; i < p.bufs.size(); ++i) {
+        const WsBuf& b = p.bufs[i];
+        long long* r = rows + 5 * i;
+        r[0] = (long long)b.off; r[1] = (long long)b.bytes; r[2] = b.first; r[3] = b.last; r[4] = b.tapped;
+      }
+    }
+    return (long long)p.bytes;
   } catch (const sgmse::Error& err) { sgmse::set_last_error(err.msg); return -1; }
   catch (...) { sgmse::set_last_error("unknown error"); return -1; }
 }
@@ -1962,7 +2069,7 @@ int sgmse_b200_set_option(sgmse_b200_engine* e, const char* key, long long value
     SG_CHECK(value == 0 || value == 5, "tc_variant %lld: 0 (TMA-fed convolutions, separate GroupNorm passes) or 5 (GroupNorm+SiLU fused into the convolutions)", value);
     e->opts.tc_variant = (int)value;
     if (e->lanes.size() > 1) ensure_lanes(*e, 1);
-    e->arena_need.clear();
+    e->ws_plans.clear();
     clear_graphs(*e);
   }
   else if (k == "attn_variant") { e->opts.attn_variant = (int)value; clear_graphs(*e); }
@@ -1970,12 +2077,24 @@ int sgmse_b200_set_option(sgmse_b200_engine* e, const char* key, long long value
   else if (k == "inconv_variant") { e->opts.inconv_variant = (int)value; clear_graphs(*e); }
   else if (k == "combine_variant") { e->opts.combine_variant = (int)value; clear_graphs(*e); }
   else if (k == "tc1_narrow") { e->opts.tc1_narrow = (int)value; clear_graphs(*e); }
-  else if (k == "gn_self") { e->opts.gn_self = (int)value; clear_graphs(*e); }
+  else if (k == "gn_self") {
+    e->opts.gn_self = (int)value;               // skips or keeps the finalize launches: changes the plan's steps
+    if (e->lanes.size() > 1) ensure_lanes(*e, 1);
+    e->ws_plans.clear();
+    clear_graphs(*e);
+  }
+  else if (k == "workspace_poison") {
+    // test option: fill each buffer with 0xFF bytes (NaN in fp16 and fp32) right after its last reader is enqueued, so
+    // that a read past a buffer's planned lifetime shows up as NaN; captured graphs are re-captured with the fills
+    e->workspace_poison = value != 0;
+    for (Engine* l : e->lanes) l->workspace_poison = e->workspace_poison;
+    clear_graphs(*e);
+  }
   else if (k == "gnfin_variant") { e->opts.gnfin_variant = (int)value; clear_graphs(*e); }
   else if (k == "outconv_variant") {
     e->opts.outconv_variant = (int)value;       // changes the buffers a forward needs (fused GroupNorm or not)
     if (e->lanes.size() > 1) ensure_lanes(*e, 1);
-    e->arena_need.clear();
+    e->ws_plans.clear();
     clear_graphs(*e);
   }
   else if (k == "pdl") {
@@ -1997,7 +2116,7 @@ int sgmse_b200_set_option(sgmse_b200_engine* e, const char* key, long long value
   else if (k == "tc_mask") {
     e->tc_mask = value;
     if (e->lanes.size() > 1) ensure_lanes(*e, 1);
-    e->arena_need.clear();
+    e->ws_plans.clear();
     clear_graphs(*e);
   }
   else SG_CHECK(false, "unknown option '%s'", key);

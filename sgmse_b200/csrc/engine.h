@@ -2,6 +2,8 @@
 #pragma once
 #include <cufft.h>
 
+#include <algorithm>
+#include <climits>
 #include <map>
 #include <memory>
 #include <string>
@@ -49,19 +51,60 @@ struct Layer {
   uint2* small_wfrag = nullptr;   // LK_OUTCONV: mma.sync B fragments [9][C/16][32] of small_w in fp16 (see out_conv_mma_kernel)
 };
 
+// One buffer of a forward pass's workspace: where it lies in the arena and the launch steps between which it is live.
+// Step s is the s-th launch of the forward; a buffer is live from the step that follows its allocation to the launch
+// of its last reader.  `last == steps` (one past the last launch): the buffer is read after the forward returns.
+struct WsBuf {
+  size_t off = 0, bytes = 0;
+  int first = 0, last = 0;
+  bool tapped = false;     // recorded as a tap (record_taps): kept to the end so that get_tap can read it
+};
+
+struct WsPlan {
+  std::vector<WsBuf> bufs;                 // in allocation order
+  std::vector<std::vector<int>> ends;      // [step]: buffers whose last reader is that launch (workspace_poison)
+  int steps = 0;                           // launches of one forward
+  size_t bytes = 0;                        // arena bytes the layout needs
+  size_t bump = 0;                         // bytes without reuse: every buffer in its own 256-B aligned range
+};
+
+// Workspace of one forward pass.  Planning mode (dry): alloc() hands out stand-in addresses and records each buffer's
+// size; use() extends the lifetime of the buffer holding an address to the current step.  Run mode: alloc() hands out
+// the planned addresses in allocation order.
 struct Arena {
+  static constexpr uintptr_t kStandIn = (uintptr_t)1 << 56;   // above every device address
   uint8_t* base = nullptr;
-  size_t cap = 0, off = 0, high = 0;
+  size_t cap = 0;
   bool dry = false;
+  int step = 0;
+  size_t off = 0;                          // planning: bump offset of the next stand-in address
+  std::vector<WsBuf> rec;                  // planning: buffers so far (off = stand-in offset)
+  const WsPlan* plan = nullptr;            // run
+  size_t next = 0;                         // run: index of the next buffer of the plan
+
+  void begin(const WsPlan* p) { step = 0; off = 0; next = 0; rec.clear(); plan = p; }
   void* alloc(size_t bytes) {
-    off = (off + 255) & ~(size_t)255;
-    void* p = base ? base + off : reinterpret_cast<void*>(off);
-    off += bytes;
-    if (off > high) high = off;
-    if (!dry) SG_CHECK(off <= cap, "workspace overflow: need %zu, have %zu", off, cap);
-    return p;
+    if (dry) {
+      off = (off + 255) & ~(size_t)255;
+      rec.push_back(WsBuf{off, bytes, step, step, false});
+      void* p = reinterpret_cast<void*>(kStandIn + off);
+      off += bytes;
+      return p;
+    }
+    SG_CHECK(plan && next < plan->bufs.size() && plan->bufs[next].bytes == bytes,
+             "internal: forward allocation %zu (%zu bytes) departs from its workspace plan", next, bytes);
+    const WsBuf& b = plan->bufs[next++];
+    SG_CHECK(b.off + b.bytes <= cap, "workspace overflow: need %zu, have %zu", b.off + b.bytes, cap);
+    return base + b.off;
   }
-  void reset() { off = 0; }
+  WsBuf* find(const void* p) {
+    const uintptr_t a = reinterpret_cast<uintptr_t>(p);
+    if (!dry || a < kStandIn || a >= kStandIn + off) return nullptr;
+    auto it = std::upper_bound(rec.begin(), rec.end(), (size_t)(a - kStandIn), [](size_t o, const WsBuf& b) { return o < b.off; });
+    return it == rec.begin() ? nullptr : &*(it - 1);
+  }
+  void use(const void* p) { if (WsBuf* b = find(p)) b->last = std::max(b->last, step); }
+  void keep(const void* p, bool tap) { if (WsBuf* b = find(p)) { b->last = INT_MAX; b->tapped |= tap; } }
 };
 
 struct GraphKey {
@@ -146,7 +189,8 @@ struct sgmse_b200_engine {
   int max_graphs = 16;                        // a long-running service sees many (B, T, sampler) keys: keep the 16 most recent
   std::map<std::tuple<int, int, int>, sgmse::FwdGraph> fwd_graphs;   // (B, F, T) -> captured single evaluation
   sgmse::OdeBuffers ode;
-  std::map<std::tuple<int, int, int>, size_t> arena_need;   // workspace bytes per (B, F, T)
+  std::map<std::tuple<int, int, int, bool>, sgmse::WsPlan> ws_plans;   // workspace layout per (B, F, T, record_taps)
+  bool workspace_poison = false;              // fill each buffer with 0xFF bytes after its last reader (test option)
   cudaStream_t own_stream = nullptr;
   std::map<std::pair<int, int>, cufftHandle> fft_plans;   // (type<<28 | n_fft, batch)
   void* stft_buf[4] = {nullptr, nullptr, nullptr, nullptr};

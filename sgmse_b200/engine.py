@@ -465,10 +465,28 @@ class Engine:
         _lib.check(self.lib.sgmse_b200_set_option(self._h, key.encode(), int(value)))
 
     def workspace_bytes(self, B: int, F: int, T: int) -> int:
+        """Bytes of all activation buffers of one forward of (B, F, T) without reuse.  The engine allocates
+        ``workspace_plan(B, F, T)["bytes"]``."""
         n = int(self.lib.sgmse_b200_workspace_bytes(self._h, B, F, T))
         if n < 0:
             _lib.check(1)
         return n
+
+    def workspace_plan(self, B: int, F: int, T: int) -> dict:
+        """The activation workspace of one forward of (B, F, T) with the current options, host-only:
+        ``{"bytes": allocated bytes, "steps": launches of the forward, "buffers": int64 [n, 5]}`` with one row
+        (offset, bytes, first step, last step, tapped) per buffer in allocation order.  ``last == steps``: the buffer
+        is read after the forward returns (the output pyramid, and with ``record_taps`` every tapped tensor)."""
+        import numpy as np
+        n, steps = C.c_longlong(), C.c_int()
+        if self.lib.sgmse_b200_workspace_plan(self._h, B, F, T, None, 0, C.byref(n), C.byref(steps)) < 0:
+            _lib.check(1)
+        rows = np.zeros((n.value, 5), dtype=np.int64)
+        nbytes = int(self.lib.sgmse_b200_workspace_plan(self._h, B, F, T, rows.ctypes.data, n.value, C.byref(n),
+                                                        C.byref(steps)))
+        if nbytes < 0:
+            _lib.check(1)
+        return {"bytes": nbytes, "steps": int(steps.value), "buffers": rows}
 
     def counter(self, key: str) -> int:
         return int(self.lib.sgmse_b200_get_counter(self._h, key.encode()))
