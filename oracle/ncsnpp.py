@@ -31,7 +31,7 @@ def fir_down2(x: torch.Tensor) -> torch.Tensor:
     """downsample_2d(x, (1,3,3,1), factor=2): pad 1/1, 4x4 FIR, keep every 2nd
     (up_or_down_sampling.py:227-257 -> upfirdn2d(down=2, pad=(1,1)))."""
     B, C, H, W = x.shape
-    k = fir_kernel_2d(x.dtype).view(1, 1, 4, 4)
+    k = fir_kernel_2d(x.dtype).to(x.device).view(1, 1, 4, 4)
     y = F.conv2d(F.pad(x.reshape(B * C, 1, H, W), (1, 1, 1, 1)), k, stride=2)
     return y.view(B, C, H // 2, W // 2)
 
@@ -42,7 +42,7 @@ def fir_up2(x: torch.Tensor) -> torch.Tensor:
     B, C, H, W = x.shape
     z = x.new_zeros(B * C, 1, 2 * H, 2 * W)
     z[:, :, ::2, ::2] = x.reshape(B * C, 1, H, W)
-    k = (fir_kernel_2d(x.dtype) * 4.0).view(1, 1, 4, 4)   # symmetric: flip is a no-op
+    k = (fir_kernel_2d(x.dtype) * 4.0).to(x.device).view(1, 1, 4, 4)   # symmetric: flip is a no-op
     y = F.conv2d(F.pad(z, (2, 1, 2, 1)), k)
     return y.view(B, C, 2 * H, 2 * W)
 

@@ -402,7 +402,6 @@ __device__ __forceinline__ float silu_tanh_half_arg(float hz) {
   asm("tanh.approx.f32 %0, %1;" : "=f"(t) : "f"(hz));
   return fmaf(hz, t, hz);
 }
-__device__ __forceinline__ uint32_t h2_add(uint32_t a, uint32_t b) { uint32_t d; asm("add.rn.f16x2 %0, %1, %2;" : "=r"(d) : "r"(a), "r"(b)); return d; }
 __device__ __forceinline__ uint32_t h2_mul(uint32_t a, uint32_t b) { uint32_t d; asm("mul.rn.f16x2 %0, %1, %2;" : "=r"(d) : "r"(a), "r"(b)); return d; }
 __device__ __forceinline__ uint32_t h2_fma(uint32_t a, uint32_t b, uint32_t c) { uint32_t d; asm("fma.rn.f16x2 %0, %1, %2, %3;" : "=r"(d) : "r"(a), "r"(b), "r"(c)); return d; }
 
@@ -490,8 +489,9 @@ gn_apply_fir_tiled_kernel(const T* __restrict__ x0, int C, const float2* __restr
   }
   __syncthreads();
   if constexpr (FAST && RS == RS_DOWN) {
-    // half2 arithmetic, tree-shaped: row sums k0*(t0+t3) + k1*(t1+t2), then the same across the four rows
-    // (4 rounding levels of 2^-11 instead of 16 sequential ones; x0.125 is exact)
+    // half2 arithmetic, separable: each row k1*t2 + (k1*t1 + (k0*t3 + k0*t0)), then the same across the four rows.  Every
+    // tap is weighted before it is added, so no partial sum exceeds the largest tap: adding two taps first (t1 + t2) turns
+    // in-range values of 32760 or more into inf.  Three roundings of 2^-11 per stage (x0.125 is exact).
     const uint32_t K0 = 0x30003000u, K1 = 0x36003600u;   // half2(0.125), half2(0.375)
     for (int item = threadIdx.x; item < TOUT * TOUT * CV; item += 256) {
       const int opx = item / CV;
@@ -513,7 +513,7 @@ gn_apply_fir_tiled_kernel(const T* __restrict__ x0, int C, const float2* __restr
           const uint32_t* t3 = reinterpret_cast<const uint32_t*>(&tt[3]);
           uint32_t* rr = reinterpret_cast<uint32_t*>(&r);
 #pragma unroll
-          for (int q = 0; q < 4; ++q) rr[q] = h2_fma(K1, h2_add(t1[q], t2[q]), h2_mul(K0, h2_add(t0[q], t3[q])));
+          for (int q = 0; q < 4; ++q) rr[q] = h2_fma(K1, t2[q], h2_fma(K1, t1[q], h2_fma(K0, t3[q], h2_mul(K0, t0[q]))));
         };
         rowsum(th, rh[i]);
         rowsum(tx, rx[i]);
@@ -526,7 +526,7 @@ gn_apply_fir_tiled_kernel(const T* __restrict__ x0, int C, const float2* __restr
         const uint32_t* r3 = reinterpret_cast<const uint32_t*>(&r[3]);
         uint32_t* oo = reinterpret_cast<uint32_t*>(&o);
 #pragma unroll
-        for (int q = 0; q < 4; ++q) oo[q] = h2_fma(K1, h2_add(r1[q], r2[q]), h2_mul(K0, h2_add(r0[q], r3[q])));
+        for (int q = 0; q < 4; ++q) oo[q] = h2_fma(K1, r2[q], h2_fma(K1, r1[q], h2_fma(K0, r3[q], h2_mul(K0, r0[q]))));
       };
       colsum(rh, oh);
       colsum(rx, oxr);

@@ -112,14 +112,15 @@ def _stream():
     return torch.cuda.current_stream().cuda_stream if torch.cuda.is_available() else None
 
 
-def build_shim(outdir):
-    """Compile the shim with the library's ARCH / CFLAGS and link it against the library's own objects."""
+def build_shim(outdir, src=SHIM_SRC):
+    """Compile a shim (tests/c/*.cu) with the library's ARCH / CFLAGS and link it against the library's own objects."""
     B.build()
     objs = [os.path.join(B.LIBDIR, "obj", s.replace(".cu", ".o")) for s in B.SOURCES]
     if not all(os.path.exists(o) for o in objs):
         B.build(force=True)
-    shim_o, so = os.path.join(outdir, "kernel_ops.o"), os.path.join(outdir, "libkernel_ops.so")
-    for cmd in ([B.NVCC, *B.ARCH, *B.CFLAGS, *B.PRODUCT_DEFS, "-I", B.CSRC, "-c", SHIM_SRC, "-o", shim_o],
+    name = os.path.splitext(os.path.basename(src))[0]
+    shim_o, so = os.path.join(outdir, name + ".o"), os.path.join(outdir, f"lib{name}.so")
+    for cmd in ([B.NVCC, *B.ARCH, *B.CFLAGS, *B.PRODUCT_DEFS, "-I", B.CSRC, "-c", src, "-o", shim_o],
                 [B.NVCC, *B.ARCH, "-shared", "-cudart", "static", "-o", so, shim_o, *objs, "-L" + B.CUDA_LIB, "-lcufft",
                  "-Xlinker", "-Bsymbolic", "-Xlinker", "-rpath," + B.CUDA_LIB]):
         r = subprocess.run(cmd, capture_output=True, text=True)

@@ -16,15 +16,13 @@ import collections
 import ctypes as C
 import math
 import os
-import subprocess
 
 import numpy as np
 import pytest
 import torch
 import torch.nn.functional as F
 
-from sgmse_b200 import build as B
-from test_gpu_kernel_ops import (H100_SMS, INV_SQRT2, ULP32, Guarded, Plan, check_stats, conv_ref, emulate_conv_tc,
+from test_gpu_kernel_ops import (H100_SMS, INV_SQRT2, ULP32, Guarded, Plan, build_shim, check_stats, conv_ref, emulate_conv_tc,
                                  ratio, slot_sums)
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
@@ -77,23 +75,9 @@ class KernelOpsTf32:
         return out
 
 
-def build_shim(outdir):
-    B.build()
-    objs = [os.path.join(B.LIBDIR, "obj", s.replace(".cu", ".o")) for s in B.SOURCES]
-    if not all(os.path.exists(o) for o in objs):
-        B.build(force=True)
-    shim_o, so = os.path.join(outdir, "kernel_ops_tf32.o"), os.path.join(outdir, "libkernel_ops_tf32.so")
-    for cmd in ([B.NVCC, *B.ARCH, *B.CFLAGS, *B.PRODUCT_DEFS, "-I", B.CSRC, "-c", SHIM_SRC, "-o", shim_o],
-                [B.NVCC, *B.ARCH, "-shared", "-cudart", "static", "-o", so, shim_o, *objs, "-L" + B.CUDA_LIB, "-lcufft",
-                 "-Xlinker", "-Bsymbolic", "-Xlinker", "-rpath," + B.CUDA_LIB]):
-        r = subprocess.run(cmd, capture_output=True, text=True)
-        assert r.returncode == 0, r.stdout + r.stderr
-    return so
-
-
 @pytest.fixture(scope="module")
 def ops32(tmp_path_factory):
-    return KernelOpsTf32(build_shim(str(tmp_path_factory.mktemp("kernel_ops_tf32"))))
+    return KernelOpsTf32(build_shim(str(tmp_path_factory.mktemp("kernel_ops_tf32")), SHIM_SRC))
 
 
 # ------------------------------------------------------------------------------------------------
