@@ -28,6 +28,9 @@
  *                                    round trips :117-141), ScoreModel.get_ode_sampler model.py:370-390
  *   sgmse_b200_rk45_host             scipy.integrate.solve_ivp(method='RK45') as called at sampling/__init__.py:127-130
  *                                    (the controller sgmse_b200_ode_sample runs, on a host callback; test hook)
+ *   sgmse_b200_ode_sample_groups     ScoreModel.get_ode_sampler(minibatch=group) / per-file enhance() with the ODE
+ *                                    sampler: every `group` utterances are their own system, solved side by side
+ *   sgmse_b200_rk45_host_groups      the lockstep driver of sgmse_b200_ode_sample_groups on a host callback (test hook)
  *   sgmse_b200_analysis              _stft + _forward_transform + pad_spec sgmse/data_module.py:162-175,212-214,
  *                                    sgmse/util/other.py:76-90, model.py:435-438
  *   sgmse_b200_synthesis             to_audio (spec_back + istft) + renorm sgmse/data_module.py:177-188,216-218,
@@ -179,6 +182,26 @@ int sgmse_b200_ode_sample(sgmse_b200_engine* e, const void* y, int B, int F, int
 typedef void (*sgmse_b200_ode_rhs)(double t, const double* y, double* dydt, long long n, void* user);
 int sgmse_b200_rk45_host(sgmse_b200_ode_rhs rhs, void* user, double t0, double t_bound, double* y, long long n,
                          double rtol, double atol, int max_attempts, int* nfev, int stats[4]);
+/* Independent ODE systems side by side: y, out c64 [B,1,F,T] (device) hold ceil(B / group) systems of `group`
+ * consecutive utterances each (the last one may be shorter), 1 <= group <= max_batch.  Each system has its own RK45
+ * controller (own t, step size, accepted / rejected steps, nfe, status) and its result is bit for bit that of
+ * sgmse_b200_ode_sample on its utterances alone with utt_offset = o->utt_offset + its first utterance; prior draws are
+ * keyed by global utterance id the same way.  At most max_batch utterances are in flight, and every network evaluation
+ * of a round is batched across them; a finished system's slot goes to the next unstarted one.  A system that fails
+ * (status -1 / -2 / -3) stops alone.  nfe[systems], stats[systems][4] (as sgmse_b200_ode_sample's), info[4] =
+ * {rounds, host syncs, network forwards, utterance evaluations}: all nullable. */
+int sgmse_b200_ode_sample_groups(sgmse_b200_engine* e, const void* y, int B, int F, int T, int group, const sgmse_b200_ode* o,
+                                 const void* prior_noise, void* out, int* nfe, int* stats, long long info[4], void* stream);
+/* The lockstep driver of sgmse_b200_ode_sample_groups on a host right-hand side (host-only; works without a GPU).
+ * System i has n[i] complex128 unknowns, stored interleaved in y at the sum of the n before it (in/out).  At most
+ * `slots` systems are in flight; each round, rhs(count, systems, t, y, dydt, n, user) evaluates the `count` systems in
+ * flight that asked for an evaluation: system systems[j] at time t[j], state y[j][2 n[j]] into dydt[j].
+ * nfev[systems], stats[systems][4] and rounds are nullable. */
+typedef void (*sgmse_b200_ode_rhs_groups)(int count, const int* systems, const double* t, const double* const* y,
+                                          double* const* dydt, const long long* n, void* user);
+int sgmse_b200_rk45_host_groups(sgmse_b200_ode_rhs_groups rhs, void* user, int systems, int slots, const long long* n,
+                                double t0, double t_bound, double* y, double rtol, double atol, int max_attempts, int* nfev,
+                                int* stats, long long* rounds);
 
 /* The sampler's host-computed schedule, exactly as the captured launch sequence uses it (host-only; works without a
  * GPU): ts[N] = torch.linspace(1, t_eps, N) in fp32 (sampling/__init__.py:56), prior_std = OUVESDE._std(1)

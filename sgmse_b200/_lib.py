@@ -44,6 +44,9 @@ class Ode(C.Structure):
 
 # right-hand side of sgmse_b200_rk45_host: rhs(t, y, dydt, n, user)
 ODE_RHS = C.CFUNCTYPE(None, C.c_double, C.POINTER(C.c_double), C.POINTER(C.c_double), C.c_longlong, C.c_void_p)
+# right-hand side of sgmse_b200_rk45_host_groups: rhs(count, systems, t, y, dydt, n, user)
+ODE_RHS_GROUPS = C.CFUNCTYPE(None, C.c_int, C.POINTER(C.c_int), C.POINTER(C.c_double), C.POINTER(C.POINTER(C.c_double)),
+                             C.POINTER(C.POINTER(C.c_double)), C.POINTER(C.c_longlong), C.c_void_p)
 
 
 # every symbol include/sgmse_b200.h declares: name -> (restype, argtypes)
@@ -69,6 +72,10 @@ SYMBOLS = {
                                         C.POINTER(C.c_int * 4), _P]),
     "sgmse_b200_rk45_host": (C.c_int, [ODE_RHS, _P, C.c_double, C.c_double, _P, C.c_longlong, C.c_double, C.c_double,
                                        C.c_int, C.POINTER(C.c_int), C.POINTER(C.c_int * 4)]),
+    "sgmse_b200_ode_sample_groups": (C.c_int, [_P, _P, C.c_int, C.c_int, C.c_int, C.c_int, C.POINTER(Ode), _P, _P, _P, _P,
+                                               _P, _P]),
+    "sgmse_b200_rk45_host_groups": (C.c_int, [ODE_RHS_GROUPS, _P, C.c_int, C.c_int, _P, C.c_double, C.c_double, _P,
+                                              C.c_double, C.c_double, C.c_int, _P, _P, _P]),
     "sgmse_b200_padded_frames": (C.c_int, [_P, C.c_int]),
     "sgmse_b200_analysis": (C.c_int, [_P, _P, C.c_int, C.c_int, C.c_int, _P, _P, _P]),
     "sgmse_b200_synthesis": (C.c_int, [_P, _P, _P, C.c_int, C.c_int, C.c_int, _P, _P]),

@@ -143,7 +143,8 @@ def make_ode_sampler(engine: Engine):
     def get_ode_sampler(self, y, N=None, minibatch=None, **kwargs):
         """ScoreModel.get_ode_sampler (model.py:370-390) -> sampling.get_ode_sampler (sampling/__init__.py:72-143).
         ``N`` only lands in the copied SDE (unused by the ODE solver); ``eps`` defaults to ``t_eps`` (model.py:375).
-        Each minibatch is its own ODE system (own adaptive step sequence), as in the reference."""
+        Each minibatch is its own ODE system (own adaptive step sequence), as in the reference; with
+        minibatch <= max_batch they are solved side by side (``Engine.ode_sample_groups``)."""
         kw = dict(rtol=kwargs.get("rtol", 1e-5), atol=kwargs.get("atol", 1e-5), eps=kwargs.get("eps", engine.cfg.t_eps),
                   denoise=kwargs.get("denoise", True), method=kwargs.get("method", "RK45"),
                   seed=kwargs.get("seed", int(torch.randint(0, 2 ** 62, (1,)).item())))
@@ -158,6 +159,11 @@ def make_ode_sampler(engine: Engine):
         M = y.shape[0]
 
         def batched_sampling_fn():
+            # the minibatches solved side by side, each bit for bit as alone; an engine (or stand-in) that states no
+            # max_batch, and minibatches larger than one network evaluation, keep the loop
+            if 1 <= minibatch <= getattr(engine.cfg, "max_batch", 0):
+                with torch.no_grad():
+                    return engine.ode_sample_groups(y, group=minibatch, prior_noise=noise, **kw)
             samples, ns = [], []
             for i in range(int(ceil(M / minibatch))):
                 sl = slice(i * minibatch, (i + 1) * minibatch)

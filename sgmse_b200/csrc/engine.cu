@@ -238,6 +238,8 @@ void free_ode(Engine& e) {
   cudaFree(o.y); cudaFree(o.y_new); cudaFree(o.stage); cudaFree(o.partial);
   for (int i = 0; i < 7; ++i) cudaFree(o.k[i]);
   if (o.partial_host) cudaFreeHost(o.partial_host);
+  cudaFree(o.gpartial); cudaFree(o.rows_scale); cudaFree(o.raw);
+  if (o.gpartial_host) cudaFreeHost(o.gpartial_host);
   o = OdeBuffers{};
 }
 
@@ -246,6 +248,8 @@ void free_workspace(Engine& e) {
   e.graphs.clear();
   for (auto& g : e.fwd_graphs) cudaGraphExecDestroy(g.second.exec);
   e.fwd_graphs.clear();
+  for (auto& g : e.fwd_rows_graphs) cudaGraphExecDestroy(g.second.exec);
+  e.fwd_rows_graphs.clear();
   free_ode(e);
   for (auto& p : e.fft_plans) cufftDestroy(p.second);
   e.fft_plans.clear();
@@ -497,6 +501,10 @@ struct Fwd {
   bool dry;
   DType dt;
   float in_scale = 1.f;  // c_in of the preconditioned forward: multiplies the (x, y) state inside the input conv
+  // the input pyramid's source when it differs from `state` (state already scaled by c_in per sample), and its
+  // per-sample c_in, applied after the first FIR-down as in_scale is (device, nullable)
+  const float4* pyr_state = nullptr;
+  const float* pyr_scale_rows = nullptr;
 
   TensorDesc act(int N, int H, int W, int C, bool stats) {
     TensorDesc t;
@@ -729,7 +737,8 @@ struct Fwd {
       tap("in_conv", h0);
       hs.push_back(h0);
     }
-    const float4* pyr_in = state;
+    const float4* pyr_in = pyr_state ? pyr_state : state;
+    const float4* const pyr0 = pyr_in;
     int ph = H, pw = W;
     for (int lvl = 0; lvl < L; ++lvl) {
       for (int b = 0; b < c.num_res_blocks; ++b) {
@@ -743,7 +752,8 @@ struct Fwd {
           const Layer& l = next(LK_COMBINE);
           float4* pd = act4(B, ph / 2, pw / 2);
           // the input pyramid starts at the network input c_in * (x, y) (ncsnpp.py:293-296): the first level carries c_in
-          if (!dry) launch_fir4(st, pyr_in, B, ph, pw, RS_DOWN, pd, pyr_in == state ? in_scale : 1.f);
+          if (!dry)
+            launch_fir4(st, pyr_in, B, ph, pw, RS_DOWN, pd, pyr_in == pyr0 ? in_scale : 1.f, pyr_in == pyr0 ? pyr_scale_rows : nullptr);
           step(pyr_in, pd);
           pyr_in = pd; ph /= 2; pw /= 2;
           TensorDesc o = act(B, h.H, h.W, h.C, true);
@@ -859,6 +869,8 @@ void clear_graphs(Engine& e) {
   e.graphs.clear();
   for (auto& g : e.fwd_graphs) cudaGraphExecDestroy(g.second.exec);
   e.fwd_graphs.clear();
+  for (auto& g : e.fwd_rows_graphs) cudaGraphExecDestroy(g.second.exec);
+  e.fwd_rows_graphs.clear();
   ++e.generation;
 }
 
@@ -886,7 +898,7 @@ void ensure_lanes(Engine& e, int want) {
     l->state = nullptr; l->xmean = nullptr; l->temb_table = nullptr; l->temb_scratch = nullptr; l->t_dev = nullptr;
     l->coef_dev = nullptr; l->rng_dev = nullptr; l->lv_scratch = nullptr; l->dbg_flag = nullptr;
     l->persist_px = 0; l->persist_rows = 0;
-    l->graphs.clear(); l->fwd_graphs.clear(); l->fft_plans.clear();
+    l->graphs.clear(); l->fwd_graphs.clear(); l->fwd_rows_graphs.clear(); l->fft_plans.clear();
     l->ode = OdeBuffers{};
     for (int i = 0; i < 4; ++i) { l->stft_buf[i] = nullptr; l->stft_cap[i] = 0; }
     l->own_stream = nullptr;
@@ -1399,14 +1411,12 @@ void ensure_ode(Engine& e, size_t px) {
 // shape is captured the first time it runs (that first evaluation itself is eager) and replayed afterwards: an ODE
 // solve is hundreds of evaluations of the same sequence with nothing but t changing, and t lives in device memory
 // (temb row, drift coefficients are kernel arguments of the un-captured drift kernel).
-const float4* forward_on_state(Engine& e, int Bc, int F, int T, cudaStream_t st, float in_scale = 1.f) {
-  Fwd f{e, st, e.temb_table, 0, false, act_dtype(e.cfg)};
-  f.in_scale = in_scale;                                       // c_in(t) of a preconditioned model: a kernel argument, so
-  const bool graph_ok = e.cfg.use_graphs && !e.time_convs && !e.record_taps && st != nullptr && in_scale == 1.f;   // not graphed
-  if (!graph_ok) return f.run(e.state, Bc, F, T);
-  const auto key = std::make_tuple(Bc, F, T);
-  auto it = e.fwd_graphs.find(key);
-  if (it != e.fwd_graphs.end()) {
+template <class Key>
+const float4* run_graphed(Engine& e, std::map<Key, FwdGraph>& graphs, const Key& key, Fwd& f, const float4* state, int Bc,
+                          int F, int T, cudaStream_t st, bool graph_ok) {
+  if (!graph_ok) return f.run(state, Bc, F, T);
+  auto it = graphs.find(key);
+  if (it != graphs.end()) {
     CUDA_OK(cudaGraphLaunch(it->second.exec, st));
     ++e.graph_launches;
     e.kernel_launches += it->second.kernel_nodes;
@@ -1414,13 +1424,13 @@ const float4* forward_on_state(Engine& e, int Bc, int F, int T, cudaStream_t st,
     e.tc_convs = it->second.tc_convs; e.direct_convs = it->second.direct_convs;
     return it->second.out;
   }
-  const float4* p = f.run(e.state, Bc, F, T);                  // eager: sets function attributes, surfaces launch errors
+  const float4* p = f.run(state, Bc, F, T);                     // eager: sets function attributes, surfaces launch errors
   const long long saved = e.kernel_launches;
   cudaGraph_t g = nullptr;
   CUDA_OK(cudaStreamBeginCapture(st, cudaStreamCaptureModeThreadLocal));
   const float4* pc = nullptr;
   try {
-    pc = f.run(e.state, Bc, F, T);
+    pc = f.run(state, Bc, F, T);
   } catch (...) {
     cudaStreamEndCapture(st, &g);
     if (g) cudaGraphDestroy(g);
@@ -1434,8 +1444,41 @@ const float4* forward_on_state(Engine& e, int Bc, int F, int T, cudaStream_t st,
   const long long nodes = e.kernel_launches - saved;
   e.kernel_launches = saved;                                    // recorded, not executed
   if (pc != p) { cudaGraphExecDestroy(ge); SG_CHECK(false, "internal: workspace replay moved the network output"); }
-  e.fwd_graphs.emplace(key, FwdGraph{ge, p, nodes, e.tc_convs, e.direct_convs});
+  graphs.emplace(key, FwdGraph{ge, p, nodes, e.tc_convs, e.direct_convs});
   return p;
+}
+
+const float4* forward_on_state(Engine& e, int Bc, int F, int T, cudaStream_t st, float in_scale = 1.f) {
+  Fwd f{e, st, e.temb_table, 0, false, act_dtype(e.cfg)};
+  f.in_scale = in_scale;                                       // c_in(t) of a preconditioned model: a kernel argument, so
+  const bool graph_ok = e.cfg.use_graphs && !e.time_convs && !e.record_taps && st != nullptr && in_scale == 1.f;   // not graphed
+  return run_graphed(e, e.fwd_graphs, std::make_tuple(Bc, F, T), f, e.state, Bc, F, T, st, graph_ok);
+}
+
+// One score-network evaluation of Bc rows with their own times: e.temb_table holds one row per sample.  With
+// `scaled` (per-sample c_in of a preconditioned model) e.state holds c_in (x, y) and e.ode.raw the unscaled rows, from
+// which the input pyramid starts; c_in lives in device memory, so this family is captured too.
+const float4* forward_rows(Engine& e, int Bc, int F, int T, cudaStream_t st, bool scaled) {
+  Fwd f{e, st, e.temb_table, e.total_temb_c, false, act_dtype(e.cfg)};
+  if (scaled) { f.pyr_state = e.ode.raw; f.pyr_scale_rows = e.ode.rows_scale; }
+  const bool graph_ok = e.cfg.use_graphs && !e.time_convs && !e.record_taps && st != nullptr;
+  return run_graphed(e, e.fwd_rows_graphs, std::make_tuple(Bc, F, T, scaled), f, e.state, Bc, F, T, st, graph_ok);
+}
+
+// Drift coefficients at t (float, as the reference's vec_t), computed in double and rounded to float
+struct OdeDriftCoefs { float inv_t, cs, c_in, cx, cF; };
+OdeDriftCoefs ode_drift_coefs(const Engine& e, float tf) {
+  const sgmse_b200_config& c = e.cfg;
+  const double ls = log((double)c.sigma_max / c.sigma_min);
+  const double g = c.sigma_min * pow((double)c.sigma_max / c.sigma_min, (double)tf) * sqrt(2 * ls);   // sdes.py:188-196
+  const Precond pc = is_v2(e) ? precond(c, (double)tf) : Precond{1.0, 0.0, 0.0};   // score = a x + b F(c_in x, c_in y, t)
+  OdeDriftCoefs d;
+  d.cs = (float)(0.5 * g * g);                                  // -g^2 * score * 0.5 with score = -dnn (sdes.py:116-117)
+  d.inv_t = 1.0f / tf;
+  d.c_in = (float)pc.c_in;
+  d.cx = (float)(-(double)c.theta - 0.5 * g * g * pc.a);
+  d.cF = (float)(-0.5 * g * g * pc.b);
+  return d;
 }
 
 struct OdeDeviceOps {
@@ -1462,22 +1505,15 @@ struct OdeDeviceOps {
     CUDA_OK(cudaGetLastError());
     launch_temb(st, temb_weights(e), e.t_dev, 1, e.temb_scratch, e.temb_table);
     e.kernel_launches += 3;
-    const double ls = log((double)c.sigma_max / c.sigma_min);
-    const double g = c.sigma_min * pow((double)c.sigma_max / c.sigma_min, (double)tf) * sqrt(2 * ls);   // sdes.py:188-196
-    const float cs = (float)(0.5 * g * g);                      // -g^2 * score * 0.5 with score = -dnn (sdes.py:116-117)
-    const float inv_t = 1.0f / tf;
+    const OdeDriftCoefs d = ode_drift_coefs(e, tf);
     const bool v2 = is_v2(e);
-    const Precond pc = v2 ? precond(c, (double)tf) : Precond{1.0, 0.0, 0.0};   // score = a x + b F(c_in x, c_in y, t)
     const int mb = std::max(1, c.max_batch);
     for (int b0 = 0; b0 < B; b0 += mb) {
       const int Bc = std::min(mb, B - b0);
       launch_pack_state(st, e.ode.stage + b0 * px1, Y + b0 * px1, Bc, F, T, e.state); ++e.kernel_launches;
-      const float4* p = forward_on_state(e, Bc, F, T, st, (float)pc.c_in);
-      if (v2)
-        launch_ode_drift_affine(st, e.state, p, Bc, F, T, e.out_layer, (float)(-(double)c.theta - 0.5 * g * g * pc.a), c.theta,
-                                (float)(-0.5 * g * g * pc.b), k[slot] + b0 * px1);
-      else
-        launch_ode_drift(st, e.state, p, Bc, F, T, e.out_layer, inv_t, c.theta, cs, k[slot] + b0 * px1);
+      const float4* p = forward_on_state(e, Bc, F, T, st, d.c_in);
+      if (v2) launch_ode_drift_affine(st, e.state, p, Bc, F, T, e.out_layer, d.cx, c.theta, d.cF, k[slot] + b0 * px1);
+      else launch_ode_drift(st, e.state, p, Bc, F, T, e.out_layer, d.inv_t, c.theta, d.cs, k[slot] + b0 * px1);
       ++e.kernel_launches;
     }
   }
@@ -1540,6 +1576,180 @@ void ode_sample(Engine& e, const float2* Y, int B, int F, int T, const sgmse_b20
   if (stats) { stats[0] = r.steps; stats[1] = r.rejected; stats[2] = r.status; stats[3] = 0; }
 }
 
+// ode_sample_groups: ceil(B / group) independent ODE systems of `group` consecutive utterances each, every system
+// with its own RK45 controller (rk45::solve_groups).  At most max_batch utterances are in flight: slot k of the
+// max_batch / group slots owns region k of the y / y_new / stage / K buffers.  Per round, the norms of all systems
+// in flight are one launch per kOdeSysPerLaunch systems and ONE device-to-host copy and sync; their evaluations are
+// one combine launch, one network forward over all their utterances (one time-embedding row and c_in per utterance)
+// and one drift launch.  Every kernel does, per system, what ode_sample's kernels do for that system alone, and the
+// forward is bit-identical under any batch composition, so each system's result equals ode_sample on it alone.
+struct OdeGroupOps {
+  Engine& e;
+  const float2* Y;
+  int B, group, F, T;
+  cudaStream_t st;
+  size_t px1;
+  const sgmse_b200_ode& o;
+  const float2* prior_noise;
+  float2* out;
+  float std1;
+  bool v2;
+  struct Slot { double2 *y, *y_new; float2* k[7]; float2* stage; size_t total; };
+  std::vector<Slot> slots;
+  long long syncs = 0, evaluated_rows = 0, forwards = 0;
+
+  int first(int sys) const { return sys * group; }
+  int count(int sys) const { return std::min(group, B - sys * group); }
+  size_t size(int sys) const { return (size_t)count(sys) * px1; }
+  static OdeK kk(const Slot& s) { OdeK K; for (int i = 0; i < 7; ++i) K.k[i] = s.k[i]; return K; }
+
+  void start(int sys, int k) {                       // x(T) = y + z * std(1) of the system's utterances, as ode_sample
+    const int b0 = first(sys), n = count(sys);
+    RngParams rp{o.seed, o.utt_offset + b0, 0};
+    CUDA_OK(cudaMemcpyAsync(e.rng_dev, &rp, sizeof(rp), cudaMemcpyHostToDevice, st));
+    CUDA_OK(cudaStreamSynchronize(st));
+    launch_pack_state(st, Y + b0 * px1, Y + b0 * px1, n, F, T, e.state);
+    launch_prior(st, e.state, n, F, T, std1, prior_noise ? prior_noise + b0 * px1 : nullptr, e.rng_dev, 0);
+    launch_ode_init(st, e.state, (size_t)n * px1, slots[k].y);
+    e.kernel_launches += 3;
+    CUDA_OK(cudaStreamSynchronize(st));             // rng_dev is rewritten by the next start
+    syncs += 2;
+    slots[k].total = size(sys);
+  }
+  void norms(int n, const int* sl, const rk45::Request* q, double rtol, double atol, double* v) {
+    for (int i0 = 0; i0 < n; i0 += kOdeSysPerLaunch) {
+      const int m = std::min(kOdeSysPerLaunch, n - i0);
+      OdeSysTable tab{};
+      for (int i = 0; i < m; ++i) {
+        const Slot& s = slots[sl[i0 + i]];
+        const rk45::Request& r = q[i0 + i];
+        OdeSys& d = tab.sys[i];
+        d.y = s.y; d.y_new = s.y_new; d.K = kk(s); d.total = s.total; d.s = r.s;
+        if (r.s == 3) { for (int j = 0; j < 7; ++j) d.c.a[j] = r.a[j]; d.h = r.h; }
+      }
+      launch_ode_norm_groups(st, tab, m, rtol, atol, e.ode.gpartial + (size_t)i0 * kOdeNormBlocks); ++e.kernel_launches;
+    }
+    CUDA_OK(cudaMemcpyAsync(e.ode.gpartial_host, e.ode.gpartial, (size_t)n * kOdeNormBlocks * sizeof(double),
+                            cudaMemcpyDeviceToHost, st));
+    CUDA_OK(cudaStreamSynchronize(st));
+    ++syncs;
+    for (int i = 0; i < n; ++i) {
+      double acc = 0.0;
+      for (int b = 0; b < kOdeNormBlocks; ++b) acc += e.ode.gpartial_host[(size_t)i * kOdeNormBlocks + b];
+      v[i] = sqrt(acc / (double)slots[sl[i]].total);
+    }
+  }
+  void evals(int n, const int* sys, const int* sl, const rk45::Request* q) {
+    for (int i0 = 0; i0 < n; i0 += kOdeSysPerLaunch) {
+      const int m = std::min(kOdeSysPerLaunch, n - i0);
+      OdeSysTable tab{};
+      for (int i = 0; i < m; ++i) {
+        const Slot& s = slots[sl[i0 + i]];
+        const rk45::Request& r = q[i0 + i];
+        OdeSys& d = tab.sys[i];
+        d.y = s.y; d.y_new = r.to_new ? s.y_new : nullptr; d.K = kk(s); d.total = s.total; d.stage = s.stage; d.s = r.s; d.h = r.h;
+        for (int j = 0; j < r.s; ++j) d.c.a[j] = r.a[j];
+      }
+      launch_ode_combine_groups(st, tab, m); ++e.kernel_launches;
+    }
+    std::vector<OdeRows> tabs;
+    int R = 0;
+    for (int i = 0; i < n; ++i) {
+      const Slot& s = slots[sl[i]];
+      const float tf = (float)q[i].t;                             // vec_t = torch.ones(B) * t (sampling/__init__.py:122)
+      const OdeDriftCoefs d = ode_drift_coefs(e, tf);
+      for (int u = 0; u < count(sys[i]); ++u, ++R) {
+        if (R % kOdeRowsPerLaunch == 0) tabs.emplace_back();
+        OdeRows& t = tabs.back();
+        const int r = R % kOdeRowsPerLaunch;
+        t.x[r] = s.stage + u * px1;
+        t.y[r] = Y + (first(sys[i]) + u) * px1;
+        t.k_out[r] = s.k[q[i].s] + u * px1;
+        t.t[r] = tf;
+        t.c_in[r] = d.c_in;
+        t.c0[r] = v2 ? d.cx : d.inv_t;
+        t.c1[r] = v2 ? d.cF : d.cs;
+      }
+    }
+    for (size_t c = 0; c < tabs.size(); ++c) {
+      const int r0 = (int)c * kOdeRowsPerLaunch, m = std::min(kOdeRowsPerLaunch, R - r0);
+      launch_ode_rows_pack(st, tabs[c], m, px1, e.state + r0 * px1, v2 ? e.ode.raw + r0 * px1 : nullptr, e.t_dev + r0,
+                           e.ode.rows_scale + r0);
+      ++e.kernel_launches;
+    }
+    launch_temb(st, temb_weights(e), e.t_dev, R, e.temb_scratch, e.temb_table); e.kernel_launches += 2;
+    const float4* p = forward_rows(e, R, F, T, st, v2);
+    for (size_t c = 0; c < tabs.size(); ++c) {
+      const int r0 = (int)c * kOdeRowsPerLaunch, m = std::min(kOdeRowsPerLaunch, R - r0);
+      launch_ode_rows_drift(st, tabs[c], m, px1, (v2 ? e.ode.raw : e.state) + r0 * px1, p + r0 * px1, e.out_layer,
+                            e.cfg.theta, v2);
+      ++e.kernel_launches;
+    }
+    evaluated_rows += R;
+    ++forwards;
+  }
+  void accept(int k) { std::swap(slots[k].y, slots[k].y_new); std::swap(slots[k].k[0], slots[k].k[6]); }
+  void finish(int sys, int k, const rk45::Result&) {
+    launch_ode_finish(st, slots[k].y, slots[k].total, out + first(sys) * px1); ++e.kernel_launches;
+  }
+};
+
+// nfe[systems], stats[systems][4] = {accepted steps, rejected attempts, status, 0} (both nullable); info (nullable):
+// {rounds, host syncs, network forwards, utterance evaluations}
+void ode_sample_groups(Engine& e, const float2* Y, int B, int F, int T, int group, const sgmse_b200_ode& o,
+                       const float2* prior_noise, float2* out, int* nfe, int* stats, long long* info, cudaStream_t st_in) {
+  SG_CHECK(e.loaded, "weights not loaded");
+  SG_CHECK(e.cfg.sde_kind == SGMSE_B200_SDE_OUVE, "the probability-flow ODE sampler is implemented for the 'ouve' SDE");
+  SG_CHECK(!is_v2(e) || e.cfg.loss_type != SGMSE_B200_LOSS_DATA_PREDICTION,
+           "the probability-flow ODE sampler needs a score model (loss_type 'score_matching' or 'denoiser')");
+  SG_CHECK(o.atol >= 0 && o.rtol >= 0, "`atol` must be positive.");                      // scipy validate_tol
+  SG_CHECK(o.eps > 0 && o.eps <= 1, "eps must lie in (0, T=1]");
+  const int mb = std::max(1, e.cfg.max_batch);
+  SG_CHECK(group >= 1 && group <= mb, "group=%d: a system must fit one network evaluation (1 <= group <= max_batch=%d)", group, mb);
+  cudaStream_t st = st_in;
+  if (!st) {                                        // stream capture is illegal on the legacy default stream
+    if (!e.own_stream) CUDA_OK(cudaStreamCreate(&e.own_stream));
+    st = e.own_stream;
+  }
+  struct SyncOnExit { cudaStream_t s; bool on; ~SyncOnExit() { if (on) cudaStreamSynchronize(s); } } sync_guard{st, st_in == nullptr};
+  const int systems = (B + group - 1) / group;
+  const int nslots = std::min(mb / group, systems);
+  const size_t px1 = (size_t)F * T, slot_px = (size_t)group * px1;
+  const int rows = std::min(B, nslots * group);
+  ensure_arena(e, rows, F, T);
+  ensure_persistent(e, (size_t)rows * px1, std::max(mb, 64));
+  ensure_ode(e, (size_t)nslots * slot_px);
+  OdeBuffers& ob = e.ode;
+  if (nslots > ob.cap_slots) {
+    if (ob.gpartial) { CUDA_OK(cudaDeviceSynchronize()); cudaFree(ob.gpartial); cudaFreeHost(ob.gpartial_host); }
+    CUDA_OK(cudaMalloc((void**)&ob.gpartial, (size_t)nslots * kOdeNormBlocks * sizeof(double)));
+    CUDA_OK(cudaHostAlloc((void**)&ob.gpartial_host, (size_t)nslots * kOdeNormBlocks * sizeof(double), cudaHostAllocDefault));
+    ob.cap_slots = nslots;
+  }
+  if (!ob.rows_scale) CUDA_OK(cudaMalloc((void**)&ob.rows_scale, (size_t)std::max(mb, 64) * sizeof(float)));
+  if (is_v2(e) && (size_t)rows * px1 > ob.cap_raw_px) {   // read inside captured forwards
+    if (ob.raw) { CUDA_OK(cudaDeviceSynchronize()); cudaFree(ob.raw); }
+    CUDA_OK(cudaMalloc((void**)&ob.raw, (size_t)rows * px1 * sizeof(float4)));
+    ob.cap_raw_px = (size_t)rows * px1;
+    clear_graphs(e);
+  }
+  OdeGroupOps ops{e, Y, B, group, F, T, st, px1, o, prior_noise, out, (float)ouve_std(e.cfg, 1.0), is_v2(e), {}};
+  for (int k = 0; k < nslots; ++k) {
+    OdeGroupOps::Slot s{};
+    s.y = ob.y + k * slot_px; s.y_new = ob.y_new + k * slot_px; s.stage = ob.stage + k * slot_px;
+    for (int j = 0; j < 7; ++j) s.k[j] = ob.k[j] + k * slot_px;
+    ops.slots.push_back(s);
+  }
+  std::vector<rk45::Result> res((size_t)systems);
+  const long long rounds = rk45::solve_groups(ops, systems, nslots, 1.0, o.eps, o.rtol, o.atol,
+                                              o.max_attempts > 0 ? o.max_attempts : 100000, res.data());
+  for (int i = 0; i < systems; ++i) {
+    if (nfe) nfe[i] = res[i].nfev;
+    if (stats) { stats[4 * i] = res[i].steps; stats[4 * i + 1] = res[i].rejected; stats[4 * i + 2] = res[i].status; stats[4 * i + 3] = 0; }
+  }
+  if (info) { info[0] = rounds; info[1] = ops.syncs; info[2] = ops.forwards; info[3] = ops.evaluated_rows; }
+}
+
 // The same controller on a host callback (test hook: pins rk45.h against scipy without a GPU).
 struct OdeHostOps {
   sgmse_b200_ode_rhs rhs;
@@ -1583,6 +1793,43 @@ struct OdeHostOps {
     return rms(d, &y_new, rtol, atol);
   }
   void accept() { y.swap(y_new); k[0].swap(k[6]); }
+};
+
+// rk45::solve_groups on a host callback: each slot is an OdeHostOps, and one callback evaluates every system in flight.
+struct OdeHostGroupOps {
+  sgmse_b200_ode_rhs_groups rhs;
+  void* user;
+  const long long* n;
+  const std::vector<long long>& off;    // offset of each system's values in y (complex units)
+  double* y;
+  std::vector<OdeHostOps> slots;
+  size_t size(int sys) const { return (size_t)n[sys]; }
+  void start(int sys, int k) {
+    OdeHostOps& s = slots[k];
+    s.n = n[sys];
+    s.y.assign(y + 2 * off[sys], y + 2 * (off[sys] + n[sys]));
+    s.y_new.assign((size_t)2 * s.n, 0.0);
+    s.stage.assign((size_t)2 * s.n, 0.0);
+    for (auto& v : s.k) v.assign((size_t)2 * s.n, 0.0);
+  }
+  void norms(int m, const int* sl, const rk45::Request* q, double rtol, double atol, double* v) {
+    for (int i = 0; i < m; ++i)
+      v[i] = q[i].s == 3 ? slots[sl[i]].norm_err(q[i].a, q[i].h, rtol, atol) : slots[sl[i]].norm_init(q[i].s, rtol, atol);
+  }
+  void evals(int m, const int* sys, const int* sl, const rk45::Request* q) {
+    std::vector<double> t((size_t)m);
+    std::vector<const double*> in((size_t)m);
+    std::vector<double*> outp((size_t)m);
+    std::vector<long long> nn((size_t)m);
+    for (int i = 0; i < m; ++i) {
+      OdeHostOps& s = slots[sl[i]];
+      s.combine(q[i].s, q[i].a, q[i].h, q[i].to_new);
+      t[i] = q[i].t; in[i] = s.stage.data(); outp[i] = s.k[q[i].s].data(); nn[i] = s.n;
+    }
+    rhs(m, sys, t.data(), in.data(), outp.data(), nn.data(), user);
+  }
+  void accept(int k) { slots[k].accept(); }
+  void finish(int sys, int k, const rk45::Result&) { std::copy(slots[k].y.begin(), slots[k].y.end(), y + 2 * off[sys]); }
 };
 
 // ------------------------------------------------------------------------------------------------
@@ -1684,7 +1931,7 @@ void enhance(Engine& e, const float* wav, int B, int L, const sgmse_b200_sampler
 }
 
 // ScoreModel.enhance with sde.sampler_type == 'ode' (model.py:446-447): every utterance is its own ODE system, as
-// enhance() is called per file in the reference.
+// enhance() is called per file in the reference; the systems share each batched network evaluation (group = 1).
 void enhance_ode(Engine& e, const float* wav, int B, int L, const sgmse_b200_ode& o, int pad_mode, const float2* prior_noise,
                  float* out, bool host, int* nfe, cudaStream_t st) {
   const int Tpad = padded_frames(e, L), F = e.cfg.n_fft / 2 + 1;
@@ -1700,12 +1947,7 @@ void enhance_ode(Engine& e, const float* wav, int B, int L, const sgmse_b200_ode
   const float* wsrc = wav;
   if (host) { CUDA_OK(cudaMemcpyAsync(wav_d, wav, (size_t)B * L * 4, cudaMemcpyHostToDevice, st)); wsrc = wav_d; }
   analysis(e, wsrc, B, L, pad_mode, Y, norm, st);
-  for (int b = 0; b < B; ++b) {
-    sgmse_b200_ode ob = o;
-    ob.utt_offset = o.utt_offset + b;
-    ode_sample(e, Y + b * px1, 1, F, Tpad, ob, prior_noise ? prior_noise + b * px1 : nullptr, X + b * px1, nfe ? nfe + b : nullptr,
-               nullptr, st);
-  }
+  ode_sample_groups(e, Y, B, F, Tpad, 1, o, prior_noise, X, nfe, nullptr, nullptr, st);
   float* odst = host ? out_d : out;
   synthesis(e, X, norm, B, Tpad, L, odst, st);
   if (host) {
@@ -1944,6 +2186,38 @@ int sgmse_b200_rk45_host(sgmse_b200_ode_rhs rhs, void* user, double t0, double t
   for (long long i = 0; i < 2 * n; ++i) y[i] = ops.y[i];
   if (nfev) *nfev = r.nfev;
   if (stats) { stats[0] = r.steps; stats[1] = r.rejected; stats[2] = r.status; stats[3] = 0; }
+  API_END
+}
+
+int sgmse_b200_ode_sample_groups(sgmse_b200_engine* e, const void* y, int B, int F, int T, int group, const sgmse_b200_ode* o,
+                                 const void* prior_noise, void* out, int* nfe, int* stats, long long info[4], void* stream) {
+  API_BEGIN
+  SG_CHECK(e && y && o && out && B > 0, "bad argument");
+  activate(*e);
+  ode_sample_groups(*e, (const float2*)y, B, F, T, group, *o, (const float2*)prior_noise, (float2*)out, nfe, stats, info,
+                    (cudaStream_t)stream);
+  API_END
+}
+
+int sgmse_b200_rk45_host_groups(sgmse_b200_ode_rhs_groups rhs, void* user, int systems, int slots, const long long* n,
+                                double t0, double t_bound, double* y, double rtol, double atol, int max_attempts, int* nfev,
+                                int* stats, long long* rounds) {
+  API_BEGIN
+  SG_CHECK(rhs && n && systems > 0 && slots > 0, "bad argument");
+  SG_CHECK(atol >= 0, "`atol` must be positive.");
+  std::vector<long long> off((size_t)systems + 1, 0);
+  for (int i = 0; i < systems; ++i) { SG_CHECK(n[i] >= 0, "bad argument"); off[i + 1] = off[i] + n[i]; }
+  SG_CHECK(y || off[systems] == 0, "bad argument");
+  OdeHostGroupOps ops{rhs, user, n, off, y, {}};
+  ops.slots.resize((size_t)std::min(slots, systems), OdeHostOps{nullptr, nullptr, 0, {}, {}, {}, {}});
+  std::vector<rk45::Result> res((size_t)systems);
+  const long long r = rk45::solve_groups(ops, systems, slots, t0, t_bound, rtol, atol, max_attempts > 0 ? max_attempts : 100000,
+                                         res.data());
+  for (int i = 0; i < systems; ++i) {
+    if (nfev) nfev[i] = res[i].nfev;
+    if (stats) { stats[4 * i] = res[i].steps; stats[4 * i + 1] = res[i].rejected; stats[4 * i + 2] = res[i].status; stats[4 * i + 3] = 0; }
+  }
+  if (rounds) *rounds = r;
   API_END
 }
 

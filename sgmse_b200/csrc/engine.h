@@ -145,6 +145,13 @@ struct OdeBuffers {          // state of the probability-flow ODE sampler for on
   double* partial = nullptr; // [kOdeNormBlocks] device
   double* partial_host = nullptr;   // pinned
   size_t cap_px = 0;
+  // ode_sample_groups: y, y_new, stage and K above hold the systems in flight side by side, one region per slot
+  double* gpartial = nullptr;       // [slots][kOdeNormBlocks] device
+  double* gpartial_host = nullptr;  // pinned
+  int cap_slots = 0;
+  float* rows_scale = nullptr;      // [max_batch] c_in of each row of a batched evaluation
+  float4* raw = nullptr;            // unscaled (x, y) rows of a batched evaluation of a preconditioned model
+  size_t cap_raw_px = 0;
 };
 
 }  // namespace sgmse
@@ -188,6 +195,8 @@ struct sgmse_b200_engine {
   long long graph_clock = 0;
   int max_graphs = 16;                        // a long-running service sees many (B, T, sampler) keys: keep the 16 most recent
   std::map<std::tuple<int, int, int>, sgmse::FwdGraph> fwd_graphs;   // (B, F, T) -> captured single evaluation
+  // (B, F, T, per-sample c_in) -> captured evaluation with one time-embedding row per sample (ode_sample_groups)
+  std::map<std::tuple<int, int, int, bool>, sgmse::FwdGraph> fwd_rows_graphs;
   sgmse::OdeBuffers ode;
   std::map<std::tuple<int, int, int, bool>, sgmse::WsPlan> ws_plans;   // workspace layout per (B, F, T, record_taps)
   bool workspace_poison = false;              // fill each buffer with 0xFF bytes after its last reader (test option)

@@ -100,7 +100,8 @@ void launch_combine(cudaStream_t st, const float4* pyr, const float* w, const fl
                     TensorDesc& out);
 // 4-channel FIR resample of the input/output pyramids
 // `scale` multiplies the result (the input pyramid of a c_in-scaled network input starts from the unscaled state)
-void launch_fir4(cudaStream_t st, const float4* in, int N, int H, int W, Resample rs, float4* out, float scale = 1.f);
+void launch_fir4(cudaStream_t st, const float4* in, int N, int H, int W, Resample rs, float4* out, float scale = 1.f,
+                 const float* scale_rows = nullptr);   // scale_rows (device, nullable): one scale per sample instead
 // out4 = conv3x3_{C->4}(act) + bias (+ addend);  w [9*C][4] (device), bias: HOST pointer to 4 floats
 // gn_ab != nullptr: `act` is the RAW tensor and silu(a*x+b) is applied while staging (only when out_conv_fuses_gn(act))
 bool out_conv_fuses_gn(const TensorDesc& act);
@@ -198,6 +199,38 @@ void launch_ode_finish(cudaStream_t st, const double2* y, size_t total, float2* 
 // partial[kOdeNormBlocks]: per-block sums of |v/scale|^2, see ode.cu for the four kinds
 void launch_ode_norm(cudaStream_t st, int kind, const double2* y, const double2* y_new, const OdeK& K, const OdeCoefs& c, double h,
                      double rtol, double atol, size_t total, double* partial);
+// Independent systems side by side (ode_sample_groups).  A launch covers up to kOdeSysPerLaunch systems; each system's
+// blocks do the single-system kernels' arithmetic over its own bins (the norm in kOdeNormBlocks blocks per system).
+constexpr int kOdeSysPerLaunch = 16;
+struct OdeSys {              // combine: stage = y + (sum_{j<s} c_j K_j) h, y_new nullable;  norm: kind s, E = c
+  const double2* y;
+  double2* y_new;
+  OdeK K;
+  OdeCoefs c;
+  double h;
+  size_t total;              // bins of this system
+  float2* stage;
+  int s;
+};
+struct OdeSysTable { OdeSys sys[kOdeSysPerLaunch]; };
+void launch_ode_combine_groups(cudaStream_t st, const OdeSysTable& tab, int n);
+// partial[i * kOdeNormBlocks + b]: block b's sum of system i, as launch_ode_norm writes it for that system alone
+void launch_ode_norm_groups(cudaStream_t st, const OdeSysTable& tab, int n, double rtol, double atol, double* partial);
+// The rows (utterances) of one batched network evaluation: each row's stage x and conditioning y, where its drift
+// goes, its time, its c_in, and its drift coefficients (inv_t, cs) or, affine, (cx, cF).
+constexpr int kOdeRowsPerLaunch = 32;
+struct OdeRows {
+  const float2* x[kOdeRowsPerLaunch];
+  const float2* y[kOdeRowsPerLaunch];
+  float2* k_out[kOdeRowsPerLaunch];
+  float t[kOdeRowsPerLaunch], c_in[kOdeRowsPerLaunch], c0[kOdeRowsPerLaunch], c1[kOdeRowsPerLaunch];
+};
+// state[r] = c_in (x, y) and raw[r] = (x, y) with raw != NULL, else state[r] = (x, y); t_dev / scale_dev (nullable) get t, c_in
+void launch_ode_rows_pack(cudaStream_t st, const OdeRows& rows, int n, size_t px1, float4* state, float4* raw, float* t_dev,
+                          float* scale_dev);
+// launch_ode_drift (affine: launch_ode_drift_affine) per row, state unscaled
+void launch_ode_rows_drift(cudaStream_t st, const OdeRows& rows, int n, size_t px1, const float4* state, const float4* pyr,
+                           const OutLayer& ol, float theta, bool affine);
 
 // ---- STFT front/back end (cuFFT plans live in the engine) ----
 void launch_absmax(cudaStream_t st, const float* wav, int B, int L, float* norm);

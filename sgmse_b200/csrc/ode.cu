@@ -96,9 +96,8 @@ __global__ void ode_finish_kernel(const double2* __restrict__ y, size_t total, f
 //   kind 1: v = K0           same scale                                    (d1)
 //   kind 2: v = K1 - K0      same scale                                    (d2 * h0)
 //   kind 3: v = (sum_j E_j K_j) h,  scale = atol + max(|y|, |y_new|) rtol  (_estimate_error_norm)
-__global__ void ode_norm_kernel(int kind, const double2* __restrict__ y, const double2* __restrict__ y_new, OdeK K, OdeCoefs c,
-                                double h, double rtol, double atol, size_t total, double* __restrict__ partial) {
-  __shared__ double sh[32];
+__device__ __forceinline__ double norm_acc(int kind, const double2* __restrict__ y, const double2* __restrict__ y_new,
+                                           const OdeK& K, const OdeCoefs& c, double h, double rtol, double atol, size_t total) {
   double acc = 0.0;
   for (size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x; i < total; i += (size_t)gridDim.x * blockDim.x) {
     const double2 yy = y[i];
@@ -119,8 +118,73 @@ __global__ void ode_norm_kernel(int kind, const double2* __restrict__ y, const d
     const double a = v.x / scale, b = v.y / scale;
     acc += a * a + b * b;
   }
-  const double t = block_sum(acc, sh);
+  return acc;
+}
+
+__global__ void ode_norm_kernel(int kind, const double2* __restrict__ y, const double2* __restrict__ y_new, OdeK K, OdeCoefs c,
+                                double h, double rtol, double atol, size_t total, double* __restrict__ partial) {
+  __shared__ double sh[32];
+  const double t = block_sum(norm_acc(kind, y, y_new, K, c, h, rtol, atol, total), sh);
   if (threadIdx.x == 0) partial[blockIdx.x] = t;
+}
+
+// ---- independent systems side by side (ode_sample_groups): blockIdx.y selects the system, and each system's blocks
+// run exactly the single-system kernels' arithmetic over its own bins -- the norm in the same block partition ----
+__global__ void ode_combine_groups_kernel(const __grid_constant__ OdeSysTable tab) {
+  const OdeSys& q = tab.sys[blockIdx.y];
+  for (size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x; i < q.total; i += (size_t)gridDim.x * blockDim.x) {
+    const double2 yy = q.y[i];
+    const double2 d = lin_comb(q.K, q.c, q.s, i);
+    const double re = yy.x + d.x * q.h, im = yy.y + d.y * q.h;
+    q.stage[i] = make_float2((float)re, (float)im);
+    if (q.y_new) q.y_new[i] = make_double2(re, im);
+  }
+}
+
+__global__ void ode_norm_groups_kernel(const __grid_constant__ OdeSysTable tab, double rtol, double atol, double* __restrict__ partial) {
+  __shared__ double sh[32];
+  const OdeSys& q = tab.sys[blockIdx.y];
+  const double t = block_sum(norm_acc(q.s, q.y, q.y_new, q.K, q.c, q.h, rtol, atol, q.total), sh);
+  if (threadIdx.x == 0) partial[(size_t)blockIdx.y * gridDim.x + blockIdx.x] = t;
+}
+
+// row r of a batched evaluation: t_dev[r] = t, scale_dev[r] = c_in; state[r] = (c_in x, c_in y) of the row's stage and
+// y, raw[r] (nullable) = (x, y) unscaled
+__global__ void ode_rows_pack_kernel(const __grid_constant__ OdeRows rows, int n, size_t px1, float4* __restrict__ state,
+                                     float4* __restrict__ raw, float* __restrict__ t_dev, float* __restrict__ scale_dev) {
+  const size_t idx = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (idx < (size_t)n && t_dev) { t_dev[idx] = rows.t[idx]; scale_dev[idx] = rows.c_in[idx]; }
+  if (idx >= (size_t)n * px1) return;
+  const int r = (int)(idx / px1);
+  const size_t j = idx - (size_t)r * px1;
+  const float2 a = rows.x[r][j], b = rows.y[r][j];
+  if (raw) {
+    const float c = rows.c_in[r];
+    state[idx] = make_float4(c * a.x, c * a.y, c * b.x, c * b.y);
+    raw[idx] = make_float4(a.x, a.y, b.x, b.y);
+  } else {
+    state[idx] = make_float4(a.x, a.y, b.x, b.y);
+  }
+}
+
+// ode_drift_kernel / ode_drift_affine_kernel with the row's coefficients, scattered to the row's K slot
+template <bool AFFINE>
+__global__ void ode_rows_drift_kernel(const __grid_constant__ OdeRows rows, int n, size_t px1, const float4* __restrict__ state,
+                                      const float4* __restrict__ pyr, OutLayer ol, float theta) {
+  const size_t idx = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (idx >= (size_t)n * px1) return;
+  const int r = (int)(idx / px1);
+  const size_t j = idx - (size_t)r * px1;
+  const float4 s = state[idx];
+  if (AFFINE) {
+    const float cx = rows.c0[r], cy = theta, cF = rows.c1[r];
+    const float2 d = out_layer_ode(ol, pyr[idx], 1.0f);
+    rows.k_out[r][j] = make_float2(cx * s.x + cy * s.z + cF * d.x, cx * s.y + cy * s.w + cF * d.y);
+  } else {
+    const float inv_t = rows.c0[r], cs = rows.c1[r];
+    const float2 d = out_layer_ode(ol, pyr[idx], inv_t);
+    rows.k_out[r][j] = make_float2(theta * (s.z - s.x) + cs * d.x, theta * (s.w - s.y) + cs * d.y);
+  }
 }
 
 }  // namespace
@@ -158,6 +222,30 @@ void launch_ode_finish(cudaStream_t st, const double2* y, size_t total, float2* 
 void launch_ode_norm(cudaStream_t st, int kind, const double2* y, const double2* y_new, const OdeK& K, const OdeCoefs& c, double h,
                      double rtol, double atol, size_t total, double* partial) {
   ode_norm_kernel<<<kOdeNormBlocks, 256, 0, st>>>(kind, y, y_new, K, c, h, rtol, atol, total, partial);
+  CUDA_OK(cudaGetLastError());
+}
+
+void launch_ode_combine_groups(cudaStream_t st, const OdeSysTable& tab, int n) {
+  size_t most = 0;
+  for (int i = 0; i < n; ++i) most = std::max(most, tab.sys[i].total);
+  ode_combine_groups_kernel<<<dim3(grid_for(most, 132 * 16), n), 256, 0, st>>>(tab);
+  CUDA_OK(cudaGetLastError());
+}
+void launch_ode_norm_groups(cudaStream_t st, const OdeSysTable& tab, int n, double rtol, double atol, double* partial) {
+  ode_norm_groups_kernel<<<dim3(kOdeNormBlocks, n), 256, 0, st>>>(tab, rtol, atol, partial);
+  CUDA_OK(cudaGetLastError());
+}
+void launch_ode_rows_pack(cudaStream_t st, const OdeRows& rows, int n, size_t px1, float4* state, float4* raw, float* t_dev,
+                          float* scale_dev) {
+  const size_t total = (size_t)n * px1;
+  ode_rows_pack_kernel<<<(unsigned)((total + 255) / 256), 256, 0, st>>>(rows, n, px1, state, raw, t_dev, scale_dev);
+  CUDA_OK(cudaGetLastError());
+}
+void launch_ode_rows_drift(cudaStream_t st, const OdeRows& rows, int n, size_t px1, const float4* state, const float4* pyr,
+                           const OutLayer& ol, float theta, bool affine) {
+  const size_t total = (size_t)n * px1;
+  if (affine) ode_rows_drift_kernel<true><<<(unsigned)((total + 255) / 256), 256, 0, st>>>(rows, n, px1, state, pyr, ol, theta);
+  else ode_rows_drift_kernel<false><<<(unsigned)((total + 255) / 256), 256, 0, st>>>(rows, n, px1, state, pyr, ol, theta);
   CUDA_OK(cudaGetLastError());
 }
 

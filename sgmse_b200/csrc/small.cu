@@ -498,7 +498,8 @@ __device__ __forceinline__ void fma4(float4& a, float w, const float4& v) {
 }
 
 template <int RS>
-__global__ void fir4_kernel(const float4* __restrict__ in, int N, int Hi, int Wi, float4* __restrict__ out, float scale) {
+__global__ void fir4_kernel(const float4* __restrict__ in, int N, int Hi, int Wi, float4* __restrict__ out, float scale,
+                            const float* __restrict__ scale_rows) {
   pdl_trigger(); pdl_wait();
   const int Ho = RS == RS_DOWN ? Hi / 2 : Hi * 2, Wo = RS == RS_DOWN ? Wi / 2 : Wi * 2;
   const size_t total = (size_t)N * Ho * Wo;
@@ -519,16 +520,18 @@ __global__ void fir4_kernel(const float4* __restrict__ in, int N, int Hi, int Wi
     const int y1 = (Y & 1) ? y0 + 1 : y0 - 1, x1 = (X & 1) ? x0 + 1 : x0 - 1;
     tap(y0, x0, 0.5625f); tap(y0, x1, 0.1875f); tap(y1, x0, 0.1875f); tap(y1, x1, 0.0625f);
   }
+  if (scale_rows) scale = scale_rows[n];
   if (scale != 1.f) { acc.x *= scale; acc.y *= scale; acc.z *= scale; acc.w *= scale; }
   out[idx] = acc;
 }
 
-void launch_fir4(cudaStream_t st, const float4* in, int N, int H, int W, Resample rs, float4* out, float scale) {
+void launch_fir4(cudaStream_t st, const float4* in, int N, int H, int W, Resample rs, float4* out, float scale,
+                 const float* scale_rows) {
   SG_CHECK(rs != RS_NONE, "fir4: nothing to do");
   const size_t total = rs == RS_DOWN ? (size_t)N * (H / 2) * (W / 2) : (size_t)N * H * 2 * W * 2;
   const int grid = (int)((total + 255) / 256);
-  if (rs == RS_DOWN) launch_k(fir4_kernel<RS_DOWN>, dim3(grid), dim3(256), 0, st, in, N, H, W, out, scale);
-  else launch_k(fir4_kernel<RS_UP>, dim3(grid), dim3(256), 0, st, in, N, H, W, out, scale);
+  if (rs == RS_DOWN) launch_k(fir4_kernel<RS_DOWN>, dim3(grid), dim3(256), 0, st, in, N, H, W, out, scale, scale_rows);
+  else launch_k(fir4_kernel<RS_UP>, dim3(grid), dim3(256), 0, st, in, N, H, W, out, scale, scale_rows);
   CUDA_OK(cudaGetLastError());
 }
 

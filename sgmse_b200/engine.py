@@ -158,6 +158,41 @@ def rk45_host(fun, t_span, y0, rtol=1e-3, atol=1e-6, max_attempts=0):
     return y, int(nfev.value), {"steps": stats[0], "rejected": stats[1], "status": stats[2]}
 
 
+def rk45_host_groups(fun, t_span, y0s, slots=None, rtol=1e-3, atol=1e-6, max_attempts=0):
+    """Independent ``solve_ivp(method='RK45')`` systems side by side on the lockstep driver of
+    :meth:`Engine.ode_sample_groups` (csrc/rk45.h: solve_groups), host-only.  ``y0s``: one complex array per system;
+    at most ``slots`` (default: all) systems are in flight.  ``fun(systems, ts, ys)`` evaluates, once per round, every
+    system in flight that asks for an evaluation and returns one derivative per system.
+    Returns ``(ys, nfev list, stats list of {"steps", "rejected", "status"}, rounds)``."""
+    import numpy as np
+    lib = _lib.load()
+    y0s = [np.asarray(v).astype(np.complex128).reshape(-1) for v in y0s]
+    S = len(y0s)
+    n = np.array([v.size for v in y0s], dtype=np.int64)
+    y = np.ascontiguousarray(np.concatenate(y0s) if S else np.zeros(0, np.complex128))
+
+    def rhs(count, systems, ts, yp, dp, nn, _user):
+        ids = [int(systems[i]) for i in range(count)]
+        ys = [np.ctypeslib.as_array(yp[i], shape=(2 * nn[i],)).view(np.complex128).copy() if nn[i] else
+              np.zeros(0, np.complex128) for i in range(count)]
+        ds = fun(ids, [float(ts[i]) for i in range(count)], ys)
+        for i in range(count):
+            if nn[i]:
+                np.ctypeslib.as_array(dp[i], shape=(2 * nn[i],)).view(np.complex128)[:] = np.asarray(ds[i], dtype=np.complex128)
+
+    cb = _lib.ODE_RHS_GROUPS(rhs)
+    nfev = (C.c_int * max(S, 1))()
+    stats = (C.c_int * (4 * max(S, 1)))()
+    rounds = C.c_longlong()
+    _lib.check(lib.sgmse_b200_rk45_host_groups(cb, None, S, int(slots if slots else max(S, 1)), n.ctypes.data,
+                                               float(t_span[0]), float(t_span[1]), y.ctypes.data, float(rtol), float(atol),
+                                               int(max_attempts), nfev, stats, C.byref(rounds)))
+    off = np.concatenate([[0], np.cumsum(n)])
+    ys = [y[off[i]:off[i + 1]].copy() for i in range(S)]
+    st = [{"steps": stats[4 * i], "rejected": stats[4 * i + 1], "status": stats[4 * i + 2]} for i in range(S)]
+    return ys, [int(nfev[i]) for i in range(S)], st, int(rounds.value)
+
+
 def _stream_ptr() -> int:
     return torch.cuda.current_stream().cuda_stream
 
@@ -381,6 +416,52 @@ class Engine:
         if return_stats:
             return out, int(nfe.value), {"steps": stats[0], "rejected": stats[1], "status": stats[2]}
         return out, int(nfe.value)
+
+    def ode_sample_groups(self, y: torch.Tensor, group: int = 1, prior_noise: Optional[torch.Tensor] = None, rtol: float = 1e-5,
+                          atol: float = 1e-5, eps: Optional[float] = None, denoise: bool = True, method: str = "RK45",
+                          seed: int = 0, utt_offset: int = 0, max_attempts: int = 0, return_stats: bool = False):
+        """y c64 [B,1,F,T] -> (sample, nfe list[, stats list]): ``ceil(B / group)`` independent probability-flow ODE
+        systems of ``group`` consecutive utterances each, every one with its own RK45 controller, solved side by side
+        with each network evaluation batched across the systems in flight (at most ``max_batch`` utterances).
+        System i equals :meth:`ode_sample` of ``y[i*group:(i+1)*group]`` with ``utt_offset + i*group``, bit for bit.
+        ``group=1`` is per-file ``enhance()``; ``group=k`` is ``get_ode_sampler(minibatch=k)``.  Arguments as in
+        :meth:`ode_sample`; stats also carry ``"rounds"``, ``"syncs"``, ``"forwards"`` and ``"rows"`` (utterance
+        evaluations) of the whole call."""
+        if method != "RK45":
+            raise NotImplementedError("only scipy's default method 'RK45' is implemented on the device")
+        if denoise:
+            raise TypeError("ReverseDiffusionPredictor.update_fn() missing 1 required positional argument: 'stepsize' "
+                            "(the reference's get_ode_sampler(denoise=True) fails the same way; pass denoise=False)")
+        y = self._c64(y)
+        self._use_device()
+        B, _, F, T = y.shape
+        group = int(group)
+        o = _lib.Ode()
+        o.rtol, o.atol = float(rtol), float(atol)
+        o.eps = float(self.cfg.t_eps if eps is None else eps)
+        o.max_attempts = int(max_attempts)
+        o.seed = int(seed) & 0xFFFFFFFFFFFFFFFF
+        o.utt_offset = int(utt_offset)
+        nptr = None
+        if prior_noise is not None:
+            prior_noise = self._c64(prior_noise)
+            if tuple(prior_noise.shape) != (B, 1, F, T):
+                raise ValueError(f"prior_noise must have shape {(B, 1, F, T)}, got {tuple(prior_noise.shape)}")
+            nptr = prior_noise.data_ptr()
+        S = -(-B // group) if group > 0 else 1
+        out = torch.empty_like(y)
+        nfe = (C.c_int * S)()
+        stats = (C.c_int * (4 * S))()
+        info = (C.c_longlong * 4)()
+        _lib.check(self.lib.sgmse_b200_ode_sample_groups(self._h, y.data_ptr(), B, F, T, group, C.byref(o), nptr,
+                                                         out.data_ptr(), nfe, stats, info, _stream_ptr()))
+        nfes = [int(v) for v in nfe]
+        if return_stats:
+            st = [{"steps": stats[4 * i], "rejected": stats[4 * i + 1], "status": stats[4 * i + 2],
+                   "rounds": int(info[0]), "syncs": int(info[1]), "forwards": int(info[2]), "rows": int(info[3])}
+                  for i in range(S)]
+            return out, nfes, st
+        return out, nfes
 
     # ---- STFT chain ------------------------------------------------------------------------------
     def padded_frames(self, L: int) -> int:

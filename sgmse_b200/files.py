@@ -86,7 +86,9 @@ class DirectoryEnhancer:
     """``DirectoryEnhancer(engine)(test_dir, enhanced_dir, N=30, corrector="ald", snr=0.5, ...)`` -> (written paths, noise ids).
 
     ``engine``: ``sgmse_b200.Engine`` (or any object a ``BatchedEnhancer`` accepts: the host logic is unit-tested with a
-    stand-in).  ``window``: files per pipeline window (default 4 x the engine's micro-batch)."""
+    stand-in).  ``window``: files per pipeline window (default 4 x the engine's micro-batch).  Keywords go to
+    ``BatchedEnhancer``: ``sampler_type="ode", denoise=False, rtol=..., atol=...`` enhances with the ODE sampler, one
+    system per file as the reference's file loop solves it."""
 
     def __init__(self, engine, window: Optional[int] = None, io_workers: int = 4, max_batch: Optional[int] = None,
                  resample: Optional[Callable[[torch.Tensor, int, int], torch.Tensor]] = None, device="cuda",

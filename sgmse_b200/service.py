@@ -5,7 +5,9 @@ normalise by the clip's own peak, STFT, ``pad_spec`` to a multiple of 64 frames,
 renormalise, write.  Utterances are independent, so clips whose PADDED frame count is equal can share one sampler
 launch sequence: this module buckets clips by padded frames, runs the per-clip front end (``sgmse_b200_analysis`` with
 the clip's own length and peak), stacks the padded spectrograms of a bucket into batches for ``sgmse_b200_pc_sample``
-(PC or Schroedinger-bridge kind) and runs the per-clip back end (``sgmse_b200_synthesis``).  Every clip's result is
+(PC or Schroedinger-bridge kind) and runs the per-clip back end (``sgmse_b200_synthesis``).  With
+``sampler_type="ode"`` each bucket goes whole to ``sgmse_b200_ode_sample_groups`` with one ODE system per clip, as
+the reference's per-file ``enhance()`` solves it; the clips' network evaluations are batched.  Every clip's result is
 bit-identical to enhancing it alone with the same ``(seed, utterance id)``; the ids are assigned in processing order
 and returned.  The one sampler this cannot hold for is ``corrector='langevin'``, whose step size is a batch mean
 (correctors.py:50-52: the clips of a batch are coupled): with it every clip is sampled as a batch of its own, which
@@ -72,10 +74,19 @@ class BatchedEnhancer:
 
     def __call__(self, waves: Sequence[torch.Tensor], seed: int = 0, sr: Optional[int] = None,
                  resample: Optional[Callable[[torch.Tensor, int, int], torch.Tensor]] = None, utt_base: int = 0,
-                 noise_for: Optional[Callable[[int, int], torch.Tensor]] = None, **sampler_kw):
+                 noise_for: Optional[Callable[[int, int], torch.Tensor]] = None, sampler_type: str = "pc", **sampler_kw):
         """``utt_base``: first noise id of this call (a pipeline that feeds several calls keeps the ids of a run distinct).
         ``noise_for(clip_index, padded_frames)`` -> c64 [draws, 1, 1, F, Tpad]: injected noise per clip instead of the
-        in-kernel Philox generator (parity tests against the reference's file loop)."""
+        in-kernel Philox generator (parity tests against the reference's file loop); with the ODE sampler the one
+        prior draw, c64 [1, 1, F, Tpad].
+        ``sampler_type``: "pc" (``pc_sample`` keywords) or "ode" (``ode_sample_groups`` keywords: rtol, atol, eps,
+        denoise, method, max_attempts); every clip's result equals ``enhance_ode`` of the clip alone with its id."""
+        if sampler_type not in ("pc", "ode"):
+            raise ValueError(f"sampler_type must be 'pc' or 'ode', got {sampler_type!r}")
+        ode = sampler_type == "ode"
+        if ode and sampler_kw.get("denoise", True):
+            raise TypeError("ReverseDiffusionPredictor.update_fn() missing 1 required positional argument: 'stepsize' "
+                            "(the reference's get_ode_sampler(denoise=True) fails the same way; pass denoise=False)")
         eng = self.engine
         target_sr = int(eng.cfg.sr)
         clips = []
@@ -88,6 +99,8 @@ class BatchedEnhancer:
             clips.append(w)
         # corrector 'langevin' couples the clips of a batch (correctors.py:50-52) -> batches of one clip, as enhancement.py runs them
         max_batch = 1 if sampler_kw.get("corrector", "ald") == "langevin" else self.max_batch
+        if ode:                    # one call per bucket: a finished clip's place goes to the next one of the bucket
+            max_batch = max(1, len(clips))
         plan = plan_batches([int(w.numel()) for w in clips], eng.padded_frames, max_batch)
         outs: List[Optional[torch.Tensor]] = [None] * len(clips)
         for tp, idx in plan.batches:
@@ -98,9 +111,16 @@ class BatchedEnhancer:
                 specs.append(Y)
                 norms.append(norm)
             kw = dict(sampler_kw)
-            if noise_for is not None:
-                kw["noise"] = torch.cat([torch.as_tensor(noise_for(i, tp)).to(self.device) for i in idx], dim=1)
-            X, _ = eng.pc_sample(torch.cat(specs, dim=0), seed=seed, utt_offset=utt_base + plan.utt_id[idx[0]], **kw)
+            Ys = torch.cat(specs, dim=0)
+            if ode:
+                if noise_for is not None:
+                    kw["prior_noise"] = torch.cat([torch.as_tensor(noise_for(i, tp)).to(self.device).reshape(1, *Ys.shape[1:])
+                                                   for i in idx], dim=0)
+                X, _ = eng.ode_sample_groups(Ys, group=1, seed=seed, utt_offset=utt_base + plan.utt_id[idx[0]], **kw)
+            else:
+                if noise_for is not None:
+                    kw["noise"] = torch.cat([torch.as_tensor(noise_for(i, tp)).to(self.device) for i in idx], dim=1)
+                X, _ = eng.pc_sample(Ys, seed=seed, utt_offset=utt_base + plan.utt_id[idx[0]], **kw)
             for j, i in enumerate(idx):                     # per-clip back end (enhancement.py:95-98)
                 outs[i] = eng.synthesis(X[j:j + 1], norms[j], int(clips[i].numel()))[0]
         return outs, [utt_base + i for i in plan.utt_id]
