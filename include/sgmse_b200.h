@@ -75,6 +75,11 @@ enum { SGMSE_B200_COUT_ONE = 0, SGMSE_B200_COUT_SIGMA = 1, SGMSE_B200_COUT_INV_S
 enum { SGMSE_B200_CSKIP_ZERO = 0, SGMSE_B200_CSKIP_EDM = 1 };
 /* sampler kind: predictor-corrector (sampling/__init__.py:26-70) or the Schroedinger-bridge samplers (:145-249) */
 enum { SGMSE_B200_SAMPLER_PC = 0, SGMSE_B200_SAMPLER_SB_ODE = 1, SGMSE_B200_SAMPLER_SB_SDE = 2 };
+/* spectrogram transform of SpecsDataModule --transform_type (data_module.py:118, spec_fwd / spec_back :162-188):
+ *   EXPONENT  |z|^e e^{j arg z} * spec_factor,  inverse (|z| / spec_factor)^(1/e) e^{j arg z}   (e = spec_abs_exponent)
+ *   LOG       log(1 + |z|) e^{j arg z} * spec_factor,  inverse (exp(|z / spec_factor|) - 1) e^{j arg z}
+ *   NONE      identity both ways; spec_factor and spec_abs_exponent are ignored */
+enum { SGMSE_B200_TRANSFORM_EXPONENT = 0, SGMSE_B200_TRANSFORM_LOG = 1, SGMSE_B200_TRANSFORM_NONE = 2 };
 
 typedef struct sgmse_b200_config {
   /* backbone (kwargs of NCSNpp.__init__, ncsnpp.py:50-74) */
@@ -105,6 +110,13 @@ typedef struct sgmse_b200_config {
   /* ScoreModel attributes used by the 'ncsnpp_v2' branch of forward (model.py:52-60); ignored by the other backbones */
   int loss_type, network_scaling, c_in, c_out, c_skip;
   float sigma_data;          /* 0.1 */
+  /* SGMSE_B200_TRANSFORM_*: the transform sgmse_b200_analysis applies after the STFT and sgmse_b200_synthesis undoes
+   * before the iSTFT.  0 (EXPONENT) is the reference's default. */
+  int transform_type;
+  /* 1: the backbone was trained with --no-centered (ncsnpp.py:45-47, ncsnpp_48k.py:46-47): the forward maps its four
+   * input channels to 2x - 1 before the input conv and the input pyramid (ncsnpp.py:288-290, ncsnpp_48k.py:291-293).
+   * Backbones 'ncsnpp' and 'ncsnpp_48k' only ('ncsnpp_v2' has no such option).  0: centered, the reference's default. */
+  int not_centered;
 } sgmse_b200_config;
 
 typedef struct sgmse_b200_sampler {

@@ -24,7 +24,7 @@ class Config(C.Structure):
         ("mode", C.c_int), ("max_batch", C.c_int), ("use_graphs", C.c_int),
         ("sde_kind", C.c_int), ("sb_k", C.c_float), ("sb_c", C.c_float), ("sb_eps", C.c_float),
         ("loss_type", C.c_int), ("network_scaling", C.c_int), ("c_in", C.c_int), ("c_out", C.c_int), ("c_skip", C.c_int),
-        ("sigma_data", C.c_float),
+        ("sigma_data", C.c_float), ("transform_type", C.c_int), ("not_centered", C.c_int),
     ]
 
 

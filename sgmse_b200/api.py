@@ -36,7 +36,7 @@ def config_from_score_model(model, mode="fp16_tc", max_batch=8, use_graphs=True)
     if backbone not in ("ncsnpp", "ncsnpp_48k", "ncsnpp_v2"):
         raise NotImplementedError(f"sgmse_b200 accelerates the 'ncsnpp', 'ncsnpp_48k' and 'ncsnpp_v2' backbones, not '{backbone}'")
     for attr, want in (("resblock_type", "biggan"), ("embedding_type", "fourier"), ("skip_rescale", True),
-                       ("conditional", True), ("centered", True)):
+                       ("conditional", True)):
         if getattr(dnn, attr, want) != want:
             raise NotImplementedError(f"NCSN++ option {attr}={getattr(dnn, attr)!r} is outside the accelerated path")
     nf = dnn.nf
@@ -60,8 +60,6 @@ def config_from_score_model(model, mode="fp16_tc", max_batch=8, use_graphs=True)
             if dnn.progressive_input == "input_skip":
                 i += 1                                     # Combine
     dm = model.data_module
-    if getattr(dm, "transform_type", "exponent") != "exponent":
-        raise NotImplementedError("only transform_type='exponent' is accelerated")
     hann = torch.hann_window(dm.n_fft, periodic=True)
     window = "hann" if torch.allclose(dm.window.cpu().float(), hann, atol=1e-6) else "sqrthann"
     sde = model.sde
@@ -92,7 +90,8 @@ def config_from_score_model(model, mode="fp16_tc", max_batch=8, use_graphs=True)
         scale_by_sigma=bool(getattr(dnn, "scale_by_sigma", False)) and backbone != "ncsnpp_v2",
         t_eps=float(model.t_eps),
         n_fft=dm.n_fft, hop_length=dm.hop_length, window=window, spec_factor=float(dm.spec_factor),
-        spec_abs_exponent=float(dm.spec_abs_exponent), sr=int(getattr(model, "sr", 16000)),
+        spec_abs_exponent=float(dm.spec_abs_exponent), transform_type=getattr(dm, "transform_type", "exponent"),
+        centered=bool(getattr(dnn, "centered", True)), sr=int(getattr(model, "sr", 16000)),
         mode=mode, max_batch=max_batch, use_graphs=use_graphs, **sde_kw, **pre_kw)
 
 

@@ -732,7 +732,7 @@ struct Fwd {
     std::vector<TensorDesc> hs;
     {
       TensorDesc h0 = act(B, H, W, c.nf, true);
-      if (!dry) launch_input_conv(st, state, B, H, W, e.inconv_w_packed, e.blob_dev + e.inconv_b, h0, in_scale);
+      if (!dry) launch_input_conv(st, state, B, H, W, e.inconv_w_packed, e.blob_dev + e.inconv_b, h0, in_scale, c.not_centered != 0);
       step(h0);
       tap("in_conv", h0);
       hs.push_back(h0);
@@ -751,9 +751,11 @@ struct Fwd {
         if (c.progressive_input_skip) {
           const Layer& l = next(LK_COMBINE);
           float4* pd = act4(B, ph / 2, pw / 2);
-          // the input pyramid starts at the network input c_in * (x, y) (ncsnpp.py:293-296): the first level carries c_in
+          // the input pyramid starts at the network input c_in * (x, y) (ncsnpp.py:293-296), or 2 (x, y) - 1 when not centered
+          // (ncsnpp.py:288-290): the first level carries c_in and the mapping
           if (!dry)
-            launch_fir4(st, pyr_in, B, ph, pw, RS_DOWN, pd, pyr_in == pyr0 ? in_scale : 1.f, pyr_in == pyr0 ? pyr_scale_rows : nullptr);
+            launch_fir4(st, pyr_in, B, ph, pw, RS_DOWN, pd, pyr_in == pyr0 ? in_scale : 1.f, pyr_in == pyr0 ? pyr_scale_rows : nullptr,
+                        pyr_in == pyr0 && c.not_centered != 0);
           step(pyr_in, pd);
           pyr_in = pd; ph /= 2; pw /= 2;
           TensorDesc o = act(B, h.H, h.W, h.C, true);
@@ -1871,7 +1873,7 @@ void analysis(Engine& e, const float* wav, int B, int L, int pad_mode, float2* Y
   cufftHandle h = fft_plan(e, false, c.n_fft, B * nT);
   SG_CHECK(cufftSetStream(h, st) == CUFFT_SUCCESS, "cufftSetStream failed");
   SG_CHECK(cufftExecR2C(h, (cufftReal*)e.stft_buf[0], (cufftComplex*)e.stft_buf[1]) == CUFFT_SUCCESS, "cufftExecR2C failed");
-  launch_spec_fwd(st, (const float2*)e.stft_buf[1], B, nT, F, F, Tpad, c.spec_factor, c.spec_abs_exponent,
+  launch_spec_fwd(st, (const float2*)e.stft_buf[1], B, nT, F, F, Tpad, c.spec_factor, c.spec_abs_exponent, c.transform_type,
                   pad_mode == SGMSE_B200_PAD_REFLECTION, Y);
   e.kernel_launches += 4;
 }
@@ -1881,7 +1883,7 @@ void synthesis(Engine& e, const float2* X, const float* norm, int B, int Tpad, i
   const int F = c.n_fft / 2 + 1;
   ensure_stft_buf(e, 0, (size_t)B * Tpad * c.n_fft * 4);
   ensure_stft_buf(e, 1, (size_t)B * Tpad * F * 8);
-  launch_spec_back(st, X, B, F, Tpad, F, c.spec_factor, c.spec_abs_exponent, (float2*)e.stft_buf[1]);
+  launch_spec_back(st, X, B, F, Tpad, F, c.spec_factor, c.spec_abs_exponent, c.transform_type, (float2*)e.stft_buf[1]);
   cufftHandle h = fft_plan(e, true, c.n_fft, B * Tpad);
   SG_CHECK(cufftSetStream(h, st) == CUFFT_SUCCESS, "cufftSetStream failed");
   SG_CHECK(cufftExecC2R(h, (cufftComplex*)e.stft_buf[1], (cufftReal*)e.stft_buf[0]) == CUFFT_SUCCESS, "cufftExecC2R failed");
@@ -2004,6 +2006,11 @@ int sgmse_b200_create(const sgmse_b200_config* cfg, sgmse_b200_engine** out) {
   e->cfg = *cfg;
   if (e->cfg.max_batch <= 0) e->cfg.max_batch = 8;
   SG_CHECK(cfg->mode >= 0 && cfg->mode <= 3, "unknown mode %d", cfg->mode);
+  SG_CHECK(cfg->transform_type >= SGMSE_B200_TRANSFORM_EXPONENT && cfg->transform_type <= SGMSE_B200_TRANSFORM_NONE,
+           "unknown transform_type %d (0 exponent, 1 log, 2 none)", cfg->transform_type);
+  SG_CHECK(cfg->not_centered == 0 || cfg->not_centered == 1, "not_centered must be 0 or 1, got %d", cfg->not_centered);
+  SG_CHECK(!cfg->not_centered || cfg->backbone != SGMSE_B200_BACKBONE_NCSNPP_V2,
+           "not_centered: backbone 'ncsnpp_v2' has no --no-centered option");
   build_network(*e);                          // host only: no CUDA call before the first weights arrive
   *out = e.release();
   API_END

@@ -92,16 +92,18 @@ extern thread_local int g_tc_variant;   // 0: TMA-fed convolutions, separate gn_
                                         // convolutions where the shape allows (its producer re-evaluates every tap: 3.2x slower per benchmark step on H100)
 
 // input layer: state float4 (x.re,x.im,y.re,y.im) -> conv3x3(4->C); w [36][C] (k = tap*4+cin), bias [C]
-// in_scale multiplies the state on the way in (c_in of the preconditioned 'ncsnpp_v2' forward, model.py:284,312-319)
+// in_scale multiplies the state on the way in (c_in of the preconditioned 'ncsnpp_v2' forward, model.py:284,312-319);
+// not_centered maps every in-bounds input value x to 2x - 1 first (--no-centered, ncsnpp.py:288-290), padding stays zero
 void launch_input_conv(cudaStream_t st, const float4* state, int N, int H, int W, const float* w,
-                       const float* bias, TensorDesc& out, float in_scale = 1.f);
+                       const float* bias, TensorDesc& out, float in_scale = 1.f, bool not_centered = false);
 // Combine('sum'): out = conv1x1_{4->C}(pyr) + bias + h ; pyr float4 [N,H,W]; w [4][C]
 void launch_combine(cudaStream_t st, const float4* pyr, const float* w, const float* bias, const TensorDesc& h,
                     TensorDesc& out);
 // 4-channel FIR resample of the input/output pyramids
 // `scale` multiplies the result (the input pyramid of a c_in-scaled network input starts from the unscaled state)
 void launch_fir4(cudaStream_t st, const float4* in, int N, int H, int W, Resample rs, float4* out, float scale = 1.f,
-                 const float* scale_rows = nullptr);   // scale_rows (device, nullable): one scale per sample instead
+                 const float* scale_rows = nullptr,    // scale_rows (device, nullable): one scale per sample instead
+                 bool not_centered = false);           // RS_DOWN only: taps read 2x - 1 for x (the input pyramid's first level)
 // out4 = conv3x3_{C->4}(act) + bias (+ addend);  w [9*C][4] (device), bias: HOST pointer to 4 floats
 // gn_ab != nullptr: `act` is the RAW tensor and silu(a*x+b) is applied while staging (only when out_conv_fuses_gn(act))
 bool out_conv_fuses_gn(const TensorDesc& act);
@@ -237,9 +239,10 @@ void launch_absmax(cudaStream_t st, const float* wav, int B, int L, float* norm)
 void launch_frame(cudaStream_t st, const float* wav, const float* norm, int B, int L, int n_fft, int hop, int nT,
                   int sqrt_window, float* frames);
 void launch_spec_fwd(cudaStream_t st, const float2* spec /*[B*nT][fstride]*/, int B, int nT, int F, int fstride,
-                     int Tpad, float factor, float expo, int reflect_pad, float2* Y /*[B][F][Tpad]*/);
+                     int Tpad, float factor, float expo, int transform /* SGMSE_B200_TRANSFORM_* */, int reflect_pad,
+                     float2* Y /*[B][F][Tpad]*/);
 void launch_spec_back(cudaStream_t st, const float2* X /*[B][F][Tpad]*/, int B, int F, int Tpad, int fstride,
-                          float factor, float expo, float2* spec /*[B*Tpad][fstride]*/);
+                          float factor, float expo, int transform, float2* spec /*[B*Tpad][fstride]*/);
 void launch_overlap_add(cudaStream_t st, const float* frames, const float* norm, int B, int Tpad, int n_fft, int hop,
                         int sqrt_window, int L, float* wav);
 

@@ -4,6 +4,7 @@
 // Reference: layerspp.py:32-41 + ncsnpp.py:267-284 (time embedding), ncsnpp.py:411-418 /
 // ncsnpp_48k.py:414-424 (output layer), sdes.py:188-229, predictors.py:41-76,
 // correctors.py:37-94 (update rules), data_module.py:162-218 (STFT chain), util/other.py:76-90.
+#include "../../include/sgmse_b200.h"
 #include "kernels.h"
 
 namespace sgmse {
@@ -351,9 +352,11 @@ void launch_frame(cudaStream_t st, const float* wav, const float* norm, int B, i
   CUDA_OK(cudaGetLastError());
 }
 
-// spec_fwd (|z|^e e^{j arg z} * factor), transpose [b][t][f] -> Y[b][f][t], pad T
+// spec_fwd, transpose [b][t][f] -> Y[b][f][t], pad T.  transform (SGMSE_B200_TRANSFORM_*, data_module.py:162-175):
+// exponent |z|^e e^{j arg z} * factor, log log(1 + |z|) e^{j arg z} * factor, none z.  The phase factor is z / |z| in both
+// magnitude maps, and log(1 + a) is evaluated as the reference writes it, not as log1p.
 __global__ void spec_fwd_kernel(const float2* __restrict__ spec, int nT, int F, int fstride, int Tpad,
-                                     float factor, float expo, int reflect_pad, float2* __restrict__ Y) {
+                                     float factor, float expo, int transform, int reflect_pad, float2* __restrict__ Y) {
   const int t = blockIdx.x * blockDim.x + threadIdx.x;
   const int f = blockIdx.y, b = blockIdx.z;
   if (t >= Tpad) return;
@@ -362,44 +365,59 @@ __global__ void spec_fwd_kernel(const float2* __restrict__ spec, int nT, int F, 
   if (t >= nT) ts = reflect_pad ? (2 * nT - 2 - t) : -1;
   if (ts >= 0) {
     z = spec[((size_t)b * nT + ts) * fstride + f];
-    if (expo != 1.0f) {
+    if (transform == SGMSE_B200_TRANSFORM_EXPONENT) {
+      if (expo != 1.0f) {
+        const float mag = hypotf(z.x, z.y);
+        const float g = mag > 0.f ? powf(mag, expo) / mag : 0.f;
+        z.x *= g; z.y *= g;
+      }
+      z.x *= factor; z.y *= factor;
+    } else if (transform == SGMSE_B200_TRANSFORM_LOG) {
       const float mag = hypotf(z.x, z.y);
-      const float g = mag > 0.f ? powf(mag, expo) / mag : 0.f;
+      const float g = mag > 0.f ? logf(1.0f + mag) / mag : 0.f;
       z.x *= g; z.y *= g;
+      z.x *= factor; z.y *= factor;
     }
-    z.x *= factor; z.y *= factor;
   }
   Y[((size_t)b * F + f) * Tpad + t] = z;
 }
 void launch_spec_fwd(cudaStream_t st, const float2* spec, int B, int nT, int F, int fstride, int Tpad,
-                     float factor, float expo, int reflect_pad, float2* Y) {
+                     float factor, float expo, int transform, int reflect_pad, float2* Y) {
   dim3 grid(cdiv(Tpad, 128), F, B);
-  spec_fwd_kernel<<<grid, 128, 0, st>>>(spec, nT, F, fstride, Tpad, factor, expo, reflect_pad, Y);
+  spec_fwd_kernel<<<grid, 128, 0, st>>>(spec, nT, F, fstride, Tpad, factor, expo, transform, reflect_pad, Y);
   CUDA_OK(cudaGetLastError());
 }
 
-// spec_back ((|z|/factor)^(1/e) e^{j arg z}), transpose X[b][f][t] -> spec[(b*Tpad+t)][f]
+// spec_back, transpose X[b][f][t] -> spec[(b*Tpad+t)][f].  transform (data_module.py:177-188): exponent
+// (|z|/factor)^(1/e) e^{j arg z}, log (exp(|z/factor|) - 1) e^{j arg z} (exp(a) - 1 as written, not expm1), none z
 __global__ void spec_back_kernel(const float2* __restrict__ X, int F, int Tpad, int fstride, float factor,
-                                     float expo, float2* __restrict__ spec) {
+                                     float expo, int transform, float2* __restrict__ spec) {
   const int f = blockIdx.x * blockDim.x + threadIdx.x;
   const int t = blockIdx.y, b = blockIdx.z;
   if (f >= fstride) return;
   float2 z = make_float2(0.f, 0.f);
   if (f < F) {
     z = X[((size_t)b * F + f) * Tpad + t];
-    z.x /= factor; z.y /= factor;
-    if (expo != 1.0f) {
+    if (transform == SGMSE_B200_TRANSFORM_EXPONENT) {
+      z.x /= factor; z.y /= factor;
+      if (expo != 1.0f) {
+        const float mag = hypotf(z.x, z.y);
+        const float g = mag > 0.f ? powf(mag, 1.0f / expo) / mag : 0.f;
+        z.x *= g; z.y *= g;
+      }
+    } else if (transform == SGMSE_B200_TRANSFORM_LOG) {
+      z.x /= factor; z.y /= factor;
       const float mag = hypotf(z.x, z.y);
-      const float g = mag > 0.f ? powf(mag, 1.0f / expo) / mag : 0.f;
+      const float g = mag > 0.f ? (expf(mag) - 1.0f) / mag : 0.f;
       z.x *= g; z.y *= g;
     }
   }
   spec[((size_t)b * Tpad + t) * fstride + f] = z;
 }
 void launch_spec_back(cudaStream_t st, const float2* X, int B, int F, int Tpad, int fstride, float factor,
-                          float expo, float2* spec) {
+                          float expo, int transform, float2* spec) {
   dim3 grid(cdiv(fstride, 128), Tpad, B);
-  spec_back_kernel<<<grid, 128, 0, st>>>(X, F, Tpad, fstride, factor, expo, spec);
+  spec_back_kernel<<<grid, 128, 0, st>>>(X, F, Tpad, fstride, factor, expo, transform, spec);
   CUDA_OK(cudaGetLastError());
 }
 

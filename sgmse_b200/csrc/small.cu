@@ -18,6 +18,13 @@ __device__ __forceinline__ void oc_mma(float (&d)[4], const uint32_t (&a)[4], ui
                : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3])
                : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "r"(b0), "r"(b1));
 }
+// --no-centered backbones (ncsnpp.py:288-290): x -> 2x - 1 on the network input, in fp32 (2x is exact, so the fma rounds
+// as the reference's two operations do).  Applied to in-bounds pixels only: the reference zero-pads after the mapping.
+__device__ __forceinline__ float2 uncenter2(float2 v) { return make_float2(fmaf(2.f, v.x, -1.f), fmaf(2.f, v.y, -1.f)); }
+__device__ __forceinline__ float4 uncenter4(float4 v) {
+  return make_float4(fmaf(2.f, v.x, -1.f), fmaf(2.f, v.y, -1.f), fmaf(2.f, v.z, -1.f), fmaf(2.f, v.w, -1.f));
+}
+
 // ------------------------------------------------------------------------------------------------
 // input conv: state float4 [N,H,W] -> T [N,H,W,C];   w[k][c], k = tap*4 + cin
 // ------------------------------------------------------------------------------------------------
@@ -25,7 +32,7 @@ template <typename T, int TP>
 __global__ void __launch_bounds__(128) input_conv_kernel(const float4* __restrict__ state, int H, int W, int C,
                                                          const float* __restrict__ w, const float* __restrict__ bias,
                                                          T* __restrict__ out, float* __restrict__ stats, int slots,
-                                                         float in_scale) {
+                                                         float in_scale, int not_centered) {
   __shared__ __align__(16) float in[TP][36];
   const int HW = H * W;
   const int m0 = blockIdx.x * TP;
@@ -36,7 +43,10 @@ __global__ void __launch_bounds__(128) input_conv_kernel(const float4* __restric
     const int r = r0 + p;
     const int y = r / W + tap / 3 - 1, x = r % W + tap % 3 - 1;
     float4 v = make_float4(0.f, 0.f, 0.f, 0.f);
-    if ((unsigned)y < (unsigned)H && (unsigned)x < (unsigned)W) v = state[(size_t)n * HW + (size_t)y * W + x];
+    if ((unsigned)y < (unsigned)H && (unsigned)x < (unsigned)W) {
+      v = state[(size_t)n * HW + (size_t)y * W + x];
+      if (not_centered) v = uncenter4(v);
+    }
     in[p][tap * 4 + 0] = in_scale * v.x; in[p][tap * 4 + 1] = in_scale * v.y;
     in[p][tap * 4 + 2] = in_scale * v.z; in[p][tap * 4 + 3] = in_scale * v.w;
   }
@@ -84,7 +94,7 @@ template <int NT>   // NT = C / 8
 __global__ void __launch_bounds__(128) input_conv_mma_kernel(const float4* __restrict__ state, int H, int W,
                                                              const float* __restrict__ w, const float* __restrict__ bias,
                                                              __half* __restrict__ out, float* __restrict__ stats, int slots,
-                                                             int num_tiles, float in_scale) {
+                                                             int num_tiles, float in_scale, int not_centered) {
   constexpr int C = NT * 8;
   constexpr int PITCH = C + 8;                       // halfs per staged row: conflict-free 32-bit writes, 16-B aligned rows
   pdl_trigger();                                     // weights / bias are constant: staged before pdl_wait()
@@ -132,8 +142,10 @@ __global__ void __launch_bounds__(128) input_conv_mma_kernel(const float4* __res
           float2 v = make_float2(0.f, 0.f);
           if (tap < 9) {
             const int y = py + tap / 3 - 1, x = px + tap % 3 - 1;
-            if ((unsigned)y < (unsigned)H && (unsigned)x < (unsigned)W)
+            if ((unsigned)y < (unsigned)H && (unsigned)x < (unsigned)W) {
               v = reinterpret_cast<const float2*>(sp + (size_t)y * W + x)[t & 1];
+              if (not_centered) v = uncenter2(v);
+            }
           }
           const __half2 hv = __floats2half2_rn(in_scale * v.x, in_scale * v.y);
           af[q >> 1][(q & 1) * 2 + hr] = *reinterpret_cast<const uint32_t*>(&hv);
@@ -198,7 +210,7 @@ template <int NT, bool PREFETCH>   // NT = C / 8; the separate copy keeps the ve
 __global__ void __launch_bounds__(128) input_conv_mma_pf_kernel(const float4* __restrict__ state, int H, int W,
                                                              const float* __restrict__ w, const float* __restrict__ bias,
                                                              __half* __restrict__ out, float* __restrict__ stats, int slots,
-                                                             int num_tiles, float in_scale) {
+                                                             int num_tiles, float in_scale, int not_centered) {
   constexpr int C = NT * 8;
   constexpr int PITCH = C + 8;                       // halfs per staged row: conflict-free 32-bit writes, 16-B aligned rows
   pdl_trigger();                                     // weights / bias are constant: staged before pdl_wait()
@@ -241,8 +253,10 @@ __global__ void __launch_bounds__(128) input_conv_mma_pf_kernel(const float4* __
         float2 v = make_float2(0.f, 0.f);
         if (tap < 9) {
           const int y = py + tap / 3 - 1, x = px + tap % 3 - 1;
-          if ((unsigned)y < (unsigned)H && (unsigned)x < (unsigned)W)
+          if ((unsigned)y < (unsigned)H && (unsigned)x < (unsigned)W) {
             v = reinterpret_cast<const float2*>(sp + (size_t)y * W + x)[t & 1];
+            if (not_centered) v = uncenter2(v);
+          }
         }
         raw[hr * 6 + q] = v;
       }
@@ -333,39 +347,40 @@ __global__ void __launch_bounds__(128) input_conv_mma_pf_kernel(const float4* __
 
 template <int NT, bool PREFETCH = false>
 static void input_conv_mma_launch(cudaStream_t st, const float4* state, int N, int H, int W, const float* w,
-                                  const float* bias, TensorDesc& out, float in_scale) {
+                                  const float* bias, TensorDesc& out, float in_scale, int not_centered) {
   constexpr int C = NT * 8;
   const int num_tiles = N * H * W / 128;
   const size_t smem = (size_t)3 * NT * 32 * sizeof(uint2) + (size_t)4 * 32 * (C + 8) * 2 + (size_t)4 * C * 2 * 4;
   auto k = PREFETCH ? input_conv_mma_pf_kernel<NT, true> : input_conv_mma_kernel<NT>;
   CUDA_OK(cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
   const int grid = std::min(num_tiles, 132 * 4);
-  launch_k(k, dim3(grid), dim3(128), smem, st, state, H, W, w, bias, (__half*)out.p, out.stats, out.slots, num_tiles, in_scale);
+  launch_k(k, dim3(grid), dim3(128), smem, st, state, H, W, w, bias, (__half*)out.p, out.stats, out.slots, num_tiles, in_scale, not_centered);
   CUDA_OK(cudaGetLastError());
 }
 
 void launch_input_conv(cudaStream_t st, const float4* state, int N, int H, int W, const float* w,
-                       const float* bias, TensorDesc& out, float in_scale) {
+                       const float* bias, TensorDesc& out, float in_scale, bool not_centered) {
+  const int nc = not_centered ? 1 : 0;
   const int HW = H * W;
   SG_CHECK(HW % 32 == 0, "input conv: H*W must be a multiple of 32");
   if (out.dt == DT_F16 && g_inconv_variant == 2 && HW % 128 == 0 && (out.C == 128 || out.C == 64 || out.C == 32)) {
     out.slots = HW / 128;
-    if (out.C == 128) input_conv_mma_launch<16, true>(st, state, N, H, W, w, bias, out, in_scale);
-    else if (out.C == 64) input_conv_mma_launch<8, true>(st, state, N, H, W, w, bias, out, in_scale);
-    else input_conv_mma_launch<4, true>(st, state, N, H, W, w, bias, out, in_scale);
+    if (out.C == 128) input_conv_mma_launch<16, true>(st, state, N, H, W, w, bias, out, in_scale, nc);
+    else if (out.C == 64) input_conv_mma_launch<8, true>(st, state, N, H, W, w, bias, out, in_scale, nc);
+    else input_conv_mma_launch<4, true>(st, state, N, H, W, w, bias, out, in_scale, nc);
     return;
   }
   if (out.dt == DT_F16 && g_inconv_variant == 0 && HW % 128 == 0 && (out.C == 128 || out.C == 64 || out.C == 32)) {
     out.slots = HW / 128;
-    if (out.C == 128) input_conv_mma_launch<16>(st, state, N, H, W, w, bias, out, in_scale);
-    else if (out.C == 64) input_conv_mma_launch<8>(st, state, N, H, W, w, bias, out, in_scale);
-    else input_conv_mma_launch<4>(st, state, N, H, W, w, bias, out, in_scale);
+    if (out.C == 128) input_conv_mma_launch<16>(st, state, N, H, W, w, bias, out, in_scale, nc);
+    else if (out.C == 64) input_conv_mma_launch<8>(st, state, N, H, W, w, bias, out, in_scale, nc);
+    else input_conv_mma_launch<4>(st, state, N, H, W, w, bias, out, in_scale, nc);
     return;
   }
   const int TP = (HW % 128 == 0) ? 128 : 32;
   out.slots = HW / TP;
   const int grid = N * HW / TP;
-#define GO(T, TP_) input_conv_kernel<T, TP_><<<grid, 128, 0, st>>>(state, H, W, out.C, w, bias, (T*)out.p, out.stats, out.slots, in_scale)
+#define GO(T, TP_) input_conv_kernel<T, TP_><<<grid, 128, 0, st>>>(state, H, W, out.C, w, bias, (T*)out.p, out.stats, out.slots, in_scale, nc)
   if (out.dt == DT_F16) { if (TP == 128) GO(__half, 128); else GO(__half, 32); }
   else { if (TP == 128) GO(float, 128); else GO(float, 32); }
 #undef GO
@@ -499,7 +514,7 @@ __device__ __forceinline__ void fma4(float4& a, float w, const float4& v) {
 
 template <int RS>
 __global__ void fir4_kernel(const float4* __restrict__ in, int N, int Hi, int Wi, float4* __restrict__ out, float scale,
-                            const float* __restrict__ scale_rows) {
+                            const float* __restrict__ scale_rows, int not_centered) {
   pdl_trigger(); pdl_wait();
   const int Ho = RS == RS_DOWN ? Hi / 2 : Hi * 2, Wo = RS == RS_DOWN ? Wi / 2 : Wi * 2;
   const size_t total = (size_t)N * Ho * Wo;
@@ -508,7 +523,10 @@ __global__ void fir4_kernel(const float4* __restrict__ in, int N, int Hi, int Wi
   const int X = (int)(idx % Wo), Y = (int)((idx / Wo) % Ho), n = (int)(idx / ((size_t)Wo * Ho));
   float4 acc = make_float4(0.f, 0.f, 0.f, 0.f);
   auto tap = [&](int y, int x, float w) {
-    if ((unsigned)y < (unsigned)Hi && (unsigned)x < (unsigned)Wi) fma4(acc, w, in[((size_t)n * Hi + y) * Wi + x]);
+    if ((unsigned)y < (unsigned)Hi && (unsigned)x < (unsigned)Wi) {
+      const float4 v = in[((size_t)n * Hi + y) * Wi + x];
+      fma4(acc, w, not_centered ? uncenter4(v) : v);
+    }
   };
   if (RS == RS_DOWN) {
 #pragma unroll
@@ -526,12 +544,14 @@ __global__ void fir4_kernel(const float4* __restrict__ in, int N, int Hi, int Wi
 }
 
 void launch_fir4(cudaStream_t st, const float4* in, int N, int H, int W, Resample rs, float4* out, float scale,
-                 const float* scale_rows) {
+                 const float* scale_rows, bool not_centered) {
   SG_CHECK(rs != RS_NONE, "fir4: nothing to do");
+  SG_CHECK(!not_centered || rs == RS_DOWN, "fir4: the input mapping belongs to the input pyramid's FIR-down");
   const size_t total = rs == RS_DOWN ? (size_t)N * (H / 2) * (W / 2) : (size_t)N * H * 2 * W * 2;
   const int grid = (int)((total + 255) / 256);
-  if (rs == RS_DOWN) launch_k(fir4_kernel<RS_DOWN>, dim3(grid), dim3(256), 0, st, in, N, H, W, out, scale, scale_rows);
-  else launch_k(fir4_kernel<RS_UP>, dim3(grid), dim3(256), 0, st, in, N, H, W, out, scale, scale_rows);
+  if (rs == RS_DOWN) launch_k(fir4_kernel<RS_DOWN>, dim3(grid), dim3(256), 0, st, in, N, H, W, out, scale, scale_rows,
+                                 not_centered ? 1 : 0);
+  else launch_k(fir4_kernel<RS_UP>, dim3(grid), dim3(256), 0, st, in, N, H, W, out, scale, scale_rows, 0);
   CUDA_OK(cudaGetLastError());
 }
 

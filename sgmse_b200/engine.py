@@ -27,6 +27,7 @@ C_IN = {"1": 0, "edm": 1}
 C_OUT = {"1": 0, "sigma": 1, "1/sigma": 2, "edm": 3}
 C_SKIP = {"0": 0, "edm": 1}
 SAMPLER_KINDS = {"pc": 0, "sb_ode": 1, "sb_sde": 2}
+TRANSFORMS = {"exponent": 0, "log": 1, "none": 2}
 
 
 def _lookup(table: Dict[str, int], name: str, what: str) -> int:
@@ -56,6 +57,7 @@ class EngineConfig:
     window: str = "hann"
     spec_factor: float = 0.15
     spec_abs_exponent: float = 0.5
+    transform_type: str = "exponent"               # SpecsDataModule --transform_type (data_module.py:118): 'exponent' | 'log' | 'none'
     sr: int = 16000
     mode: str = "fp16_tc"
     max_batch: int = 8
@@ -72,6 +74,8 @@ class EngineConfig:
     c_out: str = "1"
     c_skip: str = "0"
     sigma_data: float = 0.1
+    # NCSNpp / NCSNpp_48k --no-centered (ncsnpp.py:45-47): the network maps its input to 2x - 1 (ncsnpp.py:288-290)
+    centered: bool = True
 
     @staticmethod
     def ncsnpp_v2(**kw) -> "EngineConfig":
@@ -131,6 +135,10 @@ class EngineConfig:
         c.c_out = _lookup(C_OUT, self.c_out, "c_out type")
         c.c_skip = _lookup(C_SKIP, self.c_skip, "c_skip type")
         c.sigma_data = self.sigma_data
+        c.transform_type = _lookup(TRANSFORMS, self.transform_type, "Transform type")
+        if not self.centered and self.backbone == "ncsnpp_v2":
+            raise ValueError("'ncsnpp_v2' has no --no-centered option (centered must be True)")
+        c.not_centered = int(not self.centered)
         return c
 
 
